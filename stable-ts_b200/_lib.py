@@ -59,6 +59,10 @@ _SIGS = {
                                   c_void_p]),
     "stb_gemv": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_longlong,
                          c_void_p, c_void_p, c_void_p, c_longlong, c_void_p]),
+    "stb_decode_linear": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p,
+                                  c_longlong, c_void_p, c_void_p, c_void_p, c_longlong, c_void_p, c_int, c_int, c_void_p,
+                                  c_void_p, c_void_p]),
+    "stb_decode_linear_split": (c_int, [c_int, c_int]),
     "stb_split_f16": (c_int, [c_void_p, c_longlong, c_int, c_longlong, c_void_p, c_void_p, c_longlong, c_void_p]),
     "stb_model_create": (c_int, [POINTER(Dims), c_int, POINTER(c_void_p)]),
     "stb_model_destroy": (None, [c_void_p]),

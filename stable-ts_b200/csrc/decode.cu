@@ -541,7 +541,7 @@ __global__ void embed_step_kernel(const int32_t* __restrict__ tokens, const int3
     const float4* e = reinterpret_cast<const float4*>(emb + (long long)tokens[b] * d);
     const float4* p = reinterpret_cast<const float4*>(posemb + (long long)pos * d);
     float4* o = reinterpret_cast<float4*>(x + (long long)b * d);
-    float s1 = 0.f, s2 = 0.f;
+    float s1 = 0.f;
     for (int i = threadIdx.x; i < (d >> 2); i += blockDim.x) {
         const float4 a = __ldg(e + i), c = __ldg(p + i);
         const float4 v = make_float4(a.x + c.x, a.y + c.y, a.z + c.z, a.w + c.w);
@@ -551,18 +551,27 @@ __global__ void embed_step_kernel(const int32_t* __restrict__ tokens, const int3
             split_f16(v.x, h[0], l[0]); split_f16(v.y, h[1], l[1]); split_f16(v.z, h[2], l[2]); split_f16(v.w, h[3], l[3]);
             reinterpret_cast<uint2*>(xs_hi + (long long)b * d)[i] = *reinterpret_cast<const uint2*>(h);
             if (xs_lo != nullptr) reinterpret_cast<uint2*>(xs_lo + (long long)b * d)[i] = *reinterpret_cast<const uint2*>(l);
-            s1 += (v.x + v.y) + (v.z + v.w);
-            s2 += (v.x * v.x + v.y * v.y) + (v.z * v.z + v.w * v.w);
         }
+        s1 += (v.x + v.y) + (v.z + v.w);
     }
-    if (stats != nullptr) {
+    if (stats != nullptr) {                                  // (sum, sum of squares about the row mean): two passes
         __shared__ float r1[4], r2[4];
         s1 = warp_sum(s1);
-        s2 = warp_sum(s2);
-        if ((threadIdx.x & 31) == 0) { r1[threadIdx.x >> 5] = s1; r2[threadIdx.x >> 5] = s2; }
+        if ((threadIdx.x & 31) == 0) r1[threadIdx.x >> 5] = s1;
+        __syncthreads();
+        const float sum = (r1[0] + r1[1]) + (r1[2] + r1[3]);
+        const float mean = sum / (float)d;
+        float q = 0.f;
+        for (int i = threadIdx.x; i < (d >> 2); i += blockDim.x) {
+            const float4 v = o[i];                           // this thread's own stores above
+            const float a = v.x - mean, bb = v.y - mean, c = v.z - mean, w = v.w - mean;
+            q += (a * a + bb * bb) + (c * c + w * w);
+        }
+        q = warp_sum(q);
+        if ((threadIdx.x & 31) == 0) r2[threadIdx.x >> 5] = q;
         __syncthreads();
         if (threadIdx.x == 0) {
-            stats[2 * b] = (r1[0] + r1[1]) + (r1[2] + r1[3]);
+            stats[2 * b] = sum;
             stats[2 * b + 1] = (r2[0] + r2[1]) + (r2[2] + r2[3]);
         }
     }

@@ -404,7 +404,7 @@ struct StepWs {
     int* tickets;
     Split ln, attn, hid;
     Split xs;          // split planes of the raw residual stream x (LayerNorm folded into the consumer, OPT_DECODE_FUSED_LN)
-    float* stats;      // [16][B][2]: per 128-feature tile (sum, sum of squares) of every row of x
+    float* stats;      // [16][B][2]: per 128-feature tile (sum, sum of squares about the tile mean) of every row of x
     float* part;       // split-K partials [split][B][N] of the swapped wgmma decode linears
     size_t bytes;
 };
@@ -483,8 +483,11 @@ static int decode_step(stb_model* m, const int32_t* tokens, int B, int32_t* pos,
         ~PriorityScope() { launch_priority() = saved; }
     };
     // LayerNorm folded into the consumer linears (decode_linear.cu, DLFuse): only on the cluster-kernel route, only when the
-    // folded weights were supplied for every layer and the width is a whole number of 128-feature tiles
-    bool fused_ln = option(OPT_DECODE_FUSED_LN) != 0 && use_splitk && !legacy_splitk && d % 128 == 0 && d / 128 <= 16 &&
+    // folded weights were supplied for every layer and the width is a whole number of 128-feature tiles.  Only in FP16X3:
+    // with one fp16 plane the folded GEMM multiplies the raw, un-centred row, whose rounding error after centring grows
+    // as 2^-11 |mean| / std, where the LayerNorm kernels round the normalised row (2^-11)
+    bool fused_ln = option(OPT_DECODE_FUSED_LN) != 0 && m->prec == STB_PREC_FP16X3 && use_splitk && !legacy_splitk &&
+                    d % 128 == 0 && d / 128 <= 16 &&
                     t[STB_T_DEC_TOKEMB_G][0] != nullptr && t[STB_T_DEC_TOKEMB_FOLD][0] != nullptr;
     for (int l = 0; fused_ln && l < D.n_text_layer; ++l)
         for (int id = STB_L_QKV_WG; id < STB_L_COUNT; ++id)

@@ -69,7 +69,8 @@ static const OptDef g_opt_defs[OPT_COUNT] = {
     // 1: decode-step cross-attention on the warp-level tensor cores (ldmatrix + mma.sync over TMA-swizzled K / V tiles)
     {"xattn_tc", "STB_XATTN_TC", 1},
     // 1: the decode step folds every LayerNorm into the Linear that follows it (W diag(g) planes + row statistics from the
-    // producer's epilogue); needs the optional STB_L_*_WG / *_FOLD tensors, else the step runs its LayerNorm kernels
+    // producer's epilogue); needs the optional STB_L_*_WG / *_FOLD tensors, else the step runs its LayerNorm kernels.
+    // FP16X3 models only: an FP16 model's step ignores it
     {"decode_fused_ln", "STB_DECODE_FUSED_LN", 0},
 };
 static int g_opt[OPT_COUNT];
@@ -136,7 +137,7 @@ extern "C" int stb_axpby(float* y, const float* x, float a, float b, long long n
 }
 
 extern "C" const char* stb_last_error(void) { return stb::get_error(); }
-extern "C" int stb_abi_version(void) { return 2; }
+extern "C" int stb_abi_version(void) { return 3; }
 extern "C" int stb_set_option(const char* name, int value) {
     STB_REQUIRE(name, "stb_set_option: null name");
     stb::opt_init();

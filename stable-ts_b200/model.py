@@ -54,6 +54,27 @@ def _split(w: torch.Tensor, want_lo: bool):
     return hi, lo
 
 
+def fold_layernorm_into_linear(w: torch.Tensor, bias: Optional[torch.Tensor], gamma: torch.Tensor, beta: torch.Tensor,
+                               want_lo: bool):
+    """LayerNorm (gamma, beta) folded into the Linear (w [n][d], bias) that follows it, for the decode step:
+    Linear(LayerNorm(x)) = rstd (W' x - mean rowsum(W')) + (W beta + bias) with W' = W diag(gamma).  Returns the split
+    planes (hi, lo or None) of W' and fold f32 [2][n rounded up to 4] = [row sums of exactly those planes | W beta + bias].
+    The sums are taken from the fp16 planes (what the tensor core multiplies), in float64, so that `acc - mean * rowsum`
+    cancels the way the GEMM adds."""
+    w = w.float()
+    wg = w * gamma.float()[None, :]
+    hi, lo = _split(wg, want_lo)
+    rows = hi.double().sum(1) if lo is None else (hi.double() + lo.double()).sum(1)
+    cb = w.double() @ beta.double()
+    if bias is not None:
+        cb = cb + bias.double()
+    n_pad = (rows.numel() + 3) // 4 * 4                   # both vectors start 16-byte aligned (V = 51866 is not a multiple of 4)
+    fold = torch.zeros(2, n_pad, dtype=torch.float32, device=rows.device)
+    fold[0, : rows.numel()] = rows.float()
+    fold[1, : rows.numel()] = cb.float()
+    return hi, lo, fold
+
+
 def mel_filterbank(n_mels: int) -> np.ndarray:
     """librosa-style Slaney mel filterbank (sr 16 kHz, n_fft 400), the matrix whisper ships as mel_filters.npz."""
     def hz2mel(f):
@@ -91,8 +112,9 @@ class B200Whisper(WhisperProtocol):
         self._prec = {"fp16x3": L.STB_PREC_FP16X3, "fp16": L.STB_PREC_FP16}[precision]
         self._want_lo = self._prec == L.STB_PREC_FP16X3
         # also pack W diag(gamma) planes + fold vectors of the decoder linears that follow a LayerNorm: the decode step can
-        # then fold the LayerNorm into the Linear (option "decode_fused_ln"; +8 d^2 + V d weights, 1.9 GB at large-v3)
-        self.fold_layernorm = bool(fold_layernorm)
+        # then fold the LayerNorm into the Linear (option "decode_fused_ln"; +8 d^2 + V d weights, 1.9 GB at large-v3).
+        # fp16x3 only: the step never folds in fp16 (one plane of the raw row loses too much to rounding, engine.cu)
+        self.fold_layernorm = bool(fold_layernorm) and self._want_lo
         self._keep: List[torch.Tensor] = []
         self._ws: Dict[str, torch.Tensor] = {}
         self.graph_kernel_launches = 0     # kernels executed by CUDA-graph replays (the library counter only sees captures)
@@ -165,21 +187,12 @@ class B200Whisper(WhisperProtocol):
 
     def _set_folded(self, tid_w, tid_fold, is_dec, layer, w: torch.Tensor, bias: Optional[torch.Tensor], gamma: torch.Tensor,
                     beta: torch.Tensor):
-        """LayerNorm (gamma, beta) folded into the Linear (w, bias) that follows it, for the decode step (STB_L_*_WG / *_FOLD):
-        planes of W diag(gamma); fold = [row sums of exactly those planes | W beta + bias].  The sums are taken from the fp16
-        planes (what the tensor core multiplies), in float64, so that `acc - mean * rowsum` cancels the way the GEMM adds."""
-        w = w.to(self.device).float()
-        wg = w * gamma.to(self.device).float()[None, :]
-        hi, lo = _split(wg, self._want_lo)
-        rows = hi.double().sum(1) if lo is None else (hi.double() + lo.double()).sum(1)
-        cb = w.double() @ beta.to(self.device).double()
-        if bias is not None:
-            cb = cb + bias.to(self.device).double()
+        """LayerNorm (gamma, beta) folded into the Linear (w, bias) that follows it (STB_L_*_WG / *_FOLD), see
+        ``fold_layernorm_into_linear``."""
+        dev = self.device
+        hi, lo, fold = fold_layernorm_into_linear(w.to(dev), None if bias is None else bias.to(dev), gamma.to(dev), beta.to(dev),
+                                                  self._want_lo)
         self._set(tid_w, is_dec, layer, self._dev(hi), self._dev(lo) if lo is not None else None)
-        n_pad = (rows.numel() + 3) // 4 * 4                   # both vectors start 16-byte aligned (V = 51866 is not a multiple of 4)
-        fold = torch.zeros(2, n_pad, dtype=torch.float32, device=rows.device)
-        fold[0, : rows.numel()] = rows.float()
-        fold[1, : rows.numel()] = cb.float()
         self._set(tid_fold, is_dec, layer, self._dev(fold))
 
     def _pack(self, sd: Dict[str, torch.Tensor]):

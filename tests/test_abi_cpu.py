@@ -55,7 +55,7 @@ def test_option_switches_and_error_reporting_without_a_gpu():
     names are an error with a message (include/stablets_b200.h)."""
     from stable_ts_b200 import _lib as L
     lib = L.lib()
-    assert lib.stb_abi_version() >= 2
+    assert lib.stb_abi_version() >= 3
     assert L.get_option("xattn_tc") in (0, 1) and L.get_option("decode_splitk_legacy") in (0, 1)
     assert L.get_option("decode_fused_ln") in (0, 1) and L.get_option("no_such_option") == -1
     old = L.get_option("decode_splitk_legacy")
@@ -71,3 +71,5 @@ def test_option_switches_and_error_reporting_without_a_gpu():
     # argument validation happens before any CUDA call
     assert lib.stb_decode_state_bytes(None, 4) == 0 and lib.stb_decode_ws_bytes(None, 4) == 0
     assert lib.stb_axpby(None, None, 1.0, 0.0, 8, None) != 0 and b"stb_axpby" in lib.stb_last_error()
+    assert lib.stb_decode_linear(None, None, 48, 100, None, None, 1280, None, 0, None, 0, None, None, None, 1280, None, 0, 0,
+                                 None, None, None) != 0 and b"K=100" in lib.stb_last_error()
