@@ -43,13 +43,11 @@ extern "C" {
 
 STB_API const char* stb_last_error(void);
 STB_API int stb_abi_version(void);
-/* run-time switches for A/B measurement of kernel variants on the same box (defaults also from the environment: STB_<NAME>):
- *   "decode_splitk_legacy" 0/1  decode-step linears as swapped split-K GEMM + finish kernel instead of the cluster kernel;
- *   "xattn_tc"             1/0  decode-step cross-attention on ldmatrix + mma.sync over TMA-swizzled tiles / on scalar lanes;
- *   "decode_lin_priority"  1/0  greatest launch priority for the decode-step linears (matters with concurrent chains only);
+/* run-time switch for A/B measurement of a kernel variant on the same box (default also from the environment: STB_<NAME>):
  *   "decode_fused_ln"      0/1  LayerNorm folded into the decode-step linears (needs the STB_L_*_WG / *_FOLD tensors;
  *                               STB_PREC_FP16X3 models only, STB_PREC_FP16 models ignore it).
- * Unknown names are an error.  Not part of the reference's behaviour -- every setting must pass the same parity tests. */
+ * stb_set_option rejects an unknown name with an error; stb_get_option returns -1 for it.  Not part of the reference's
+ * behaviour -- every setting must pass the same parity tests. */
 STB_API int stb_set_option(const char* name, int value);
 STB_API int stb_get_option(const char* name);
 /* measurement hooks (bench.py): kernels launched by this library so far; per-launch CUDA-event timing of every kernel */
@@ -309,14 +307,12 @@ STB_API int stb_decode_step(stb_model* m, const int32_t* tokens_in, int B, int32
  *    position (positional embedding row) is pos - seq_off[b], and its self-attention reads cache rows [seq_off[b], pos] only, so
  *    every sequence samples its first token at the same step.  Steps with pos < seq_off[b] are idle for b (any token id).
  *    cache_rows: rows per sequence of the K/V caches, n_text_ctx <= cache_rows <= 2 n_text_ctx (stb_decode_state_bytes_rows).
- *    kv_total / kv_off: `cross_kv` was built by stb_cross_kv for kv_total windows and the B sequences of this call are its
- *    windows [kv_off, kv_off + B): two halves of a batch can be stepped concurrently on two streams over one block (their
- *    latency-bound linear layers then overlap the other half's HBM-bound cross-attention).  kv_total <= 0 means (B, 0).
- *    seq_off == NULL, cache_rows == n_text_ctx and kv_total == B is stb_decode_step. */
+ *    cross_kv: the block stb_cross_kv built for exactly these B windows (decode layout), sequence b reading window b.
+ *    seq_off == NULL and cache_rows == n_text_ctx is stb_decode_step. */
 STB_API size_t stb_decode_state_bytes_rows(const stb_model* m, int B, int cache_rows);
 STB_API int stb_decode_step_ragged(stb_model* m, const int32_t* tokens_in, int B, int32_t* pos, const int32_t* seq_off,
-                           int cache_rows, const void* cross_kv, int kv_total, int kv_off, void* state, float* logits_out,
-                           long long ld_logits, void* ws, size_t ws_bytes, void* stream);
+                           int cache_rows, const void* cross_kv, void* state, float* logits_out, long long ld_logits,
+                           void* ws, size_t ws_bytes, void* stream);
 
 /* per-sequence sampling state kept on the device */
 typedef struct {

@@ -86,8 +86,8 @@ _SIGS = {
     "stb_sample_greedy": (c_int, [c_void_p, c_longlong, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                   c_longlong, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "stb_decode_state_bytes_rows": (c_size_t, [c_void_p, c_int, c_int]),
-    "stb_decode_step_ragged": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p,
-                                       c_void_p, c_longlong, c_void_p, c_size_t, c_void_p]),
+    "stb_decode_step_ragged": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
+                                       c_longlong, c_void_p, c_size_t, c_void_p]),
     "stb_sample": (c_int, [c_void_p, c_longlong, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                            c_longlong, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_float, c_void_p,
                            c_void_p, c_void_p]),
@@ -137,7 +137,8 @@ def check(rc: int):
 
 
 def set_option(name: str, value: int):
-    """Run-time kernel-variant switch (stb_set_option): "decode_splitk_legacy" (A/B timing of the decode-step linears)."""
+    """Run-time kernel-variant switch (stb_set_option): "decode_fused_ln" (LayerNorm folded into the decode-step linears).
+    An unknown name raises StbError."""
     check(lib().stb_set_option(name.encode(), int(value)))
 
 

@@ -84,12 +84,13 @@ __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.lau
 
 bool pdl_enabled(int kind = 0);   // STB_PDL bit mask (misc.cu): kind 0 = ordinary kernels, 1 = decode_linear
 // run-time switches (stb_set_option / stb_get_option, misc.cu); defaults come from the environment variable of the same
-// meaning so a whole process can be flipped without code (STB_DECODE_SPLITK_LEGACY)
-enum Option { OPT_DECODE_SPLITK_LEGACY = 0, OPT_DECODE_LIN_PRIORITY, OPT_XATTN_TC, OPT_DECODE_FUSED_LN, OPT_COUNT };
+// meaning so a whole process can be flipped without code (STB_DECODE_FUSED_LN)
+enum Option { OPT_DECODE_FUSED_LN = 0, OPT_COUNT };
 int option(Option o);
 // launch priority of the kernels launched next by this host thread (cudaLaunchAttributePriority; 0 = the stream's own).
-// The decode step raises it for its latency-bound linear layers, so that -- when two half-batches are stepped on two streams --
-// the block scheduler serves a pending linear before the other half's remaining cross-attention CTAs.
+// The decode step raises it for its latency-bound linear layers: under programmatic dependent launch the next kernel's CTAs
+// can become resident while the previous kernel's tail still runs, and the block scheduler then serves the higher-priority
+// CTAs first.  Not measured against priority 0.
 int& launch_priority();
 
 template <typename... KArgs, typename... Args>

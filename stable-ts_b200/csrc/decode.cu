@@ -21,16 +21,6 @@ namespace stb {
 // exp2f (MUFU.EX2 + range fix-up) instead of expf's multiply + range reduction, executed per key by all 8 lanes of a group
 constexpr float LOG2E_F = 1.4426950408889634f;
 
-__device__ __forceinline__ void unpack8(const uint4& a, float (&f)[8]) {
-    const __half2* h = reinterpret_cast<const __half2*>(&a);
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-        const float2 t = __half22float2(h[e]);
-        f[2 * e] = t.x;
-        f[2 * e + 1] = t.y;
-    }
-}
-
 // ---------------------------------------------------------------------------------------------------------
 // self-attention over the fp32 K/V cache.  grid (H, B), 128 threads.
 //   qkv [B][3d] fp32 (q | k | v of the newest token); caches Kc, Vc [B][ctx][d] fp32; out split [B][d].
@@ -133,184 +123,26 @@ decode_self_attn_kernel(const float* __restrict__ qkv, float* __restrict__ Kc, f
 // (sequence, head) is a pair of contiguous 192 KB streams.  HBM-bound: 2 x 1500 x 128 B = 384 KB per (sequence, head) per
 // step.  The decode step reads the fp16 `hi` plane only -- K is the GEMM plane itself, V a head-major copy written once
 // per window batch.  Measured at 32 layers against the fp32 oracle (tests/test_gpu_depth.py): worst step-logit error
-// 2.15e-5 with fp16 K/V vs 2.07e-5 with the 3-byte hi + int8-residual format this kernel used before (gate 1e-3), greedy
-// tokens bit-exact -- the residual bought nothing measurable, so its 35 % of extra bytes were dropped.
+// 2.15e-5 with fp16 K/V vs 2.07e-5 with a 3-byte hi + int8-residual format (gate 1e-3), greedy tokens bit-exact -- the
+// residual bought nothing measurable, so its 35 % of extra bytes were dropped.
 //
-// Flash-decoding layout: the keys of one (b,h) are cut into XS splits.  One CTA (4 warps) owns one split: an elected thread
-// issues the split's K and V as four 1-D bulk copies (cp.async.bulk, 12 KB each) into shared memory BEFORE waiting on the
-// producer of q (programmatic dependent launch: the K/V stream does not depend on it), so with 4 CTAs per SM ~190 KB per
-// SM are in flight and the copy engine, not registers, holds the memory-level parallelism.  8 lanes share a key row
-// (one 16-byte shared load of K and of V per lane), online softmax per lane group with ONE rescale per block of 4 keys,
-// the 16 lane groups merged through shared memory; each CTA writes (m, l, acc[64]) and the last CTA of a (b,h) to finish
-// (atomic ticket) merges the XS partials and writes the output.
-// ---------------------------------------------------------------------------------------------------------
-constexpr int XS = 8;                       // key splits per (sequence, head)
-constexpr int XS_KEYS = 188;                // keys per split (8 x 188 = 1504 >= 1500)
-constexpr int XC = 2;                       // bulk-copy chunks per split (compute starts when the first one lands)
-constexpr int XC_KEYS = 94;
-constexpr int X_SMEM = XC * 2 * XC_KEYS * 128;   // K | V per chunk: 48128 B
-
-__device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar))
-                 : "memory");
-}
-
-__global__ void __launch_bounds__(128, 4)
-decode_cross_attn_kernel(const float* __restrict__ q, const __half* __restrict__ k_hi, const __half* __restrict__ v_hi, int d,
-                         int T, float* __restrict__ partial, int* __restrict__ tickets, __half* __restrict__ out_hi,
-                         __half* __restrict__ out_lo, float* __restrict__ out_f32) {
-    extern __shared__ __align__(128) uint8_t x_smem[];       // [chunk][K rows | V rows][XC_KEYS][128 B]
-    __shared__ __align__(8) uint64_t s_bar[XC];
-    __shared__ float s_m[4][4], s_l[4][4];
-    __shared__ float s_acc[4][4][64];
-    __shared__ int s_last;
-    const int split = blockIdx.x, h = blockIdx.y, b = blockIdx.z, H = gridDim.y;
-    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int sub = lane & 7, grp = lane >> 3, g16 = w * 4 + grp;
-    const int key0 = split * XS_KEYS, key1 = min(T, key0 + XS_KEYS);
-    const int nkeys = max(key1 - key0, 0);
-    if (threadIdx.x == 0) {
-#pragma unroll
-        for (int c = 0; c < XC; ++c) mbar_init(&s_bar[c], 1);
-        fence_mbar_init();
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        const long long row0 = ((long long)b * H + h) * T + key0;
-#pragma unroll
-        for (int c = 0; c < XC; ++c) {
-            const int n = min(max(nkeys - c * XC_KEYS, 0), XC_KEYS);
-            if (n > 0) {
-                const uint32_t bytes = (uint32_t)n * 128u;
-                uint8_t* dst = x_smem + (size_t)c * 2 * XC_KEYS * 128;
-                mbar_arrive_expect_tx(&s_bar[c], 2 * bytes);
-                bulk_load_1d(dst, k_hi + (row0 + c * XC_KEYS) * 64, bytes, &s_bar[c]);
-                bulk_load_1d(dst + XC_KEYS * 128, v_hi + (row0 + c * XC_KEYS) * 64, bytes, &s_bar[c]);
-            }
-        }
-    }
-    pdl_trigger();
-    pdl_wait();                                              // q comes from the preceding linear
-    float qr[8];
-#pragma unroll
-    for (int e = 0; e < 8; ++e) qr[e] = q[(long long)b * d + h * 64 + sub * 8 + e] * (0.125f * LOG2E_F);   // log2 units
-    float m = -INFINITY, l = 0.f, acc[8];
-#pragma unroll
-    for (int e = 0; e < 8; ++e) acc[e] = 0.f;
-#pragma unroll
-    for (int c = 0; c < XC; ++c) {
-        const int n = min(max(nkeys - c * XC_KEYS, 0), XC_KEYS);
-        if (n <= 0) break;
-        mbar_wait(&s_bar[c], 0, 40 + c);
-        const uint8_t* kc = x_smem + (size_t)c * 2 * XC_KEYS * 128 + sub * 16;
-        const uint8_t* vc = kc + XC_KEYS * 128;
-        // this lane group's keys of the chunk: g16 + 16 i; four at a time
-        for (int j0 = g16; j0 < n; j0 += 64) {
-            float sc[4];
-            uint4 vh[4];
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-                const int j = j0 + u * 16;
-                const bool ok = j < n;                        // uniform within the 8-lane group
-                const uint4 kh = ok ? *reinterpret_cast<const uint4*>(kc + j * 128) : make_uint4(0, 0, 0, 0);
-                vh[u] = ok ? *reinterpret_cast<const uint4*>(vc + j * 128) : make_uint4(0, 0, 0, 0);
-                float kf[8];
-                unpack8(kh, kf);
-                float s = 0.f;
-#pragma unroll
-                for (int e = 0; e < 8; ++e) s = fmaf(qr[e], kf[e], s);
-                s += __shfl_xor_sync(0xffffffffu, s, 1);
-                s += __shfl_xor_sync(0xffffffffu, s, 2);
-                s += __shfl_xor_sync(0xffffffffu, s, 4);
-                sc[u] = ok ? s : -INFINITY;
-            }
-            const float mn = fmaxf(fmaxf(m, sc[0]), fmaxf(fmaxf(sc[1], sc[2]), sc[3]));   // key u = 0 is valid: finite
-            const float corr = exp2f(m - mn);                  // exp(-inf) = 0 for the first block
-            l *= corr;
-#pragma unroll
-            for (int e = 0; e < 8; ++e) acc[e] *= corr;
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-                const float p = exp2f(sc[u] - mn);             // 0 for keys past the chunk
-                float vf[8];
-                unpack8(vh[u], vf);
-                l += p;
-#pragma unroll
-                for (int e = 0; e < 8; ++e) acc[e] = fmaf(p, vf[e], acc[e]);
-            }
-            m = mn;
-        }
-    }
-    // ---- combine the 16 lane groups of the CTA ----
-    if (sub == 0) { s_m[w][grp] = m; s_l[w][grp] = l; }
-#pragma unroll
-    for (int e = 0; e < 8; ++e) s_acc[w][grp][sub * 8 + e] = acc[e];
-    __syncthreads();
-    float* part = partial + (((long long)b * H + h) * XS + split) * 66;
-    if (threadIdx.x < 64) {
-        float M = -INFINITY;
-#pragma unroll
-        for (int i = 0; i < 16; ++i) M = fmaxf(M, s_m[i >> 2][i & 3]);
-        float Lsum = 0.f, o = 0.f;
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-            const float mi = s_m[i >> 2][i & 3];
-            const float sc = (mi == -INFINITY) ? 0.f : exp2f(mi - M);
-            Lsum += s_l[i >> 2][i & 3] * sc;
-            o += s_acc[i >> 2][i & 3][threadIdx.x] * sc;
-        }
-        part[2 + threadIdx.x] = o;
-        if (threadIdx.x == 0) { part[0] = M; part[1] = Lsum; }
-        __threadfence();                                     // (the writers only: the other two warps have nothing to publish)
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        const int t = atomicAdd(tickets + b * H + h, 1);
-        s_last = (t == XS - 1);
-        if (s_last) tickets[b * H + h] = 0;                  // re-arm for the next launch
-    }
-    __syncthreads();
-    if (s_last && threadIdx.x < 64) {
-        __threadfence();
-        const float* p0 = partial + ((long long)b * H + h) * XS * 66;
-        float M = -INFINITY;
-#pragma unroll
-        for (int i = 0; i < XS; ++i) M = fmaxf(M, __ldcg(p0 + i * 66));
-        float Lsum = 0.f, o = 0.f;
-#pragma unroll
-        for (int i = 0; i < XS; ++i) {
-            const float mi = __ldcg(p0 + i * 66);
-            const float sc = (mi == -INFINITY) ? 0.f : exp2f(mi - M);
-            Lsum += __ldcg(p0 + i * 66 + 1) * sc;
-            o += __ldcg(p0 + i * 66 + 2 + threadIdx.x) * sc;
-        }
-        o /= Lsum;
-        const long long oo = (long long)b * d + h * 64 + threadIdx.x;
-        if (out_f32) out_f32[oo] = o;
-        if (out_hi) {
-            __half hi, lo;
-            split_f16(o, hi, lo);
-            out_hi[oo] = hi;
-            if (out_lo) out_lo[oo] = lo;
-        }
-    }
-}
-
-// ---------------------------------------------------------------------------------------------------------
-// The same cross-attention on the warp-level tensor cores (option "xattn_tc").  The scalar kernel above spends ~11 warp
-// instructions per key (fp16 -> fp32 unpacking, 8-lane shuffles, one exp per lane) and runs at 62 % issue utilisation while
-// it streams; here one query row costs ~150 warp instructions per 192 keys:
+// Flash-decoding layout: grid (XS, H, B); the keys of one (b,h) are cut into XS splits of XT_CHUNKS x XT_KEYS = 192 keys
+// (8 x 192 = 1536 >= 1500).  One CTA (4 warps) owns one split: an elected thread issues the split's K and V tiles as TMA
+// copies BEFORE waiting on the producer of q (programmatic dependent launch: the K/V stream does not depend on it).  Each
+// CTA writes its partial (m, l, acc[64]) -- 66 floats at partial[((b H + h) XS + split) 66] -- and the last CTA of a (b,h)
+// to finish (atomic ticket on tickets[b H + h], re-armed to 0 for the next launch) merges the XS partials and writes the
+// output.  The arithmetic runs on the warp-level tensor cores; one query row costs ~150 warp instructions per 192 keys:
 //   * K and V tiles [96 keys][64] fp16 land through 2-D TMA copies with SWIZZLE_128B (zero fill past the last key), so
 //     ldmatrix reads them without bank conflicts;
 //   * scores: mma.sync m16n8k16, A = the query in rows 0 / 1 (fp16 hi / lo of q * log2(e) / 8: the fp32 query is
 //     represented to 2^-22), B = 8 keys per tile straight from ldmatrix; row 0 + row 1 = the fp32-grade score;
-//   * one exact softmax per CTA (max over its 192 keys through shared memory; partials of the 8 splits are merged as before);
+//   * one exact softmax per CTA (max over its 192 keys through shared memory);
 //   * P.V: mma.sync m16n8k8 per 8-key tile, A = p in rows 0 / 1 (hi / lo), B = V through ldmatrix.trans.
 // Warp w owns tiles w, w + 4, w + 8 of each 12-tile chunk.
 // (Not a persistent, double-buffered kernel: a per-item fence + ticket + barriers serialise inside a CTA, whereas 4
 //  short-lived CTAs per SM overlap each other's tails.)
 // ---------------------------------------------------------------------------------------------------------
+constexpr int XS = 8;                        // key splits per (sequence, head)
 constexpr int XT_KEYS = 96;                  // keys per chunk
 constexpr int XT_CHUNKS = 2;                 // chunks per split: 8 x 192 = 1536 >= 1500
 constexpr int XT_TILES = XT_KEYS / 8 / 4;    // 8-key tiles per warp per chunk
@@ -808,33 +640,21 @@ int decode_attn_cross(const float* q, const CrossDecodeKV& kv, int B, int H, int
     int dev = 0;
     STB_CUDA_OK(cudaGetDevice(&dev));
     if (dev >= 0 && dev < 64 && !attr_set[dev]) {
-        STB_CUDA_OK(cudaFuncSetAttribute(decode_cross_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, X_SMEM));
-        STB_CUDA_OK(cudaFuncSetAttribute(decode_cross_attn_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
+        STB_CUDA_OK(cudaFuncSetAttribute(decode_cross_attn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, XT_SMEM));
+        STB_CUDA_OK(cudaFuncSetAttribute(decode_cross_attn_tc_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
         attr_set[dev] = true;
     }
-    if (option(OPT_XATTN_TC) != 0) {
-        static bool attr_tc[64] = {};
-        if (dev >= 0 && dev < 64 && !attr_tc[dev]) {
-            STB_CUDA_OK(cudaFuncSetAttribute(decode_cross_attn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, XT_SMEM));
-            STB_CUDA_OK(cudaFuncSetAttribute(decode_cross_attn_tc_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
-            attr_tc[dev] = true;
-        }
-        const int T = (int)STB_N_AUDIO_CTX;
-        TmapVal tk, tv;
-        STB_TRY(make_tmap(kv.k_hi, T, 64, H, B, 64, (long long)T * 64, (long long)H * T * 64, XT_KEYS, &tk));
-        STB_TRY(make_tmap(kv.v_hi, T, 64, H, B, 64, (long long)T * 64, (long long)H * T * 64, XT_KEYS, &tv));
-        XPerm perm;
-        for (int i = 0; i < 3; ++i) {
-            STB_REQUIRE(tk.perm[i] == tv.perm[i], "decode_attn_cross: K / V tensor maps disagree");
-            perm.p[i] = tk.perm[i];
-        }
-        STB_CUDA_OK(launch_pdl(decode_cross_attn_tc_kernel, dim3(XS, H, B), dim3(128), (size_t)XT_SMEM, st, tk.map, tv.map, perm, q, d,
-                               T, partial, tickets, oh, ol, of));
-        STB_LAUNCH_OK();
-        return STB_OK;
+    const int T = (int)STB_N_AUDIO_CTX;
+    TmapVal tk, tv;
+    STB_TRY(make_tmap(kv.k_hi, T, 64, H, B, 64, (long long)T * 64, (long long)H * T * 64, XT_KEYS, &tk));
+    STB_TRY(make_tmap(kv.v_hi, T, 64, H, B, 64, (long long)T * 64, (long long)H * T * 64, XT_KEYS, &tv));
+    XPerm perm;
+    for (int i = 0; i < 3; ++i) {
+        STB_REQUIRE(tk.perm[i] == tv.perm[i], "decode_attn_cross: K / V tensor maps disagree");
+        perm.p[i] = tk.perm[i];
     }
-    STB_CUDA_OK(launch_pdl(decode_cross_attn_kernel, dim3(XS, H, B), dim3(128), (size_t)X_SMEM, st, q, kv.k_hi, kv.v_hi, d,
-                           (int)STB_N_AUDIO_CTX, partial, tickets, oh, ol, of));
+    STB_CUDA_OK(launch_pdl(decode_cross_attn_tc_kernel, dim3(XS, H, B), dim3(128), (size_t)XT_SMEM, st, tk.map, tv.map, perm, q, d,
+                           T, partial, tickets, oh, ol, of));
     STB_LAUNCH_OK();
     return STB_OK;
 }

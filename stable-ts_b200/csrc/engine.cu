@@ -405,23 +405,10 @@ struct StepWs {
     Split ln, attn, hid;
     Split xs;          // split planes of the raw residual stream x (LayerNorm folded into the consumer, OPT_DECODE_FUSED_LN)
     float* stats;      // [16][B][2]: per 128-feature tile (sum, sum of squares about the tile mean) of every row of x
-    float* part;       // split-K partials [split][B][N] of the swapped wgmma decode linears
     size_t bytes;
 };
-constexpr int STEP_GEMV_MAX_B = 16;      // <= : mma.sync batched GEMV; above: swapped split-K wgmma GEMM
-// tuning knobs for A/B runs (defaults carried over from the sm_100a tuning; not re-measured on an H100): STB_STEP_GEMV_MAX_B = 0..64, STB_STEP_SPLIT_TILES = 1..160
-static int env_int(const char* name, int dflt, int lo, int hi) {
-    const char* e = getenv(name);
-    if (e == nullptr || e[0] == 0) return dflt;
-    const int v = atoi(e);
-    return v < lo ? lo : v > hi ? hi : v;
-}
-static int step_gemv_max_b() {
-    static const int v = env_int("STB_STEP_GEMV_MAX_B", STEP_GEMV_MAX_B, 0, 64);
-    return v;
-}
+constexpr int STEP_GEMV_MAX_B = 16;      // <= : mma.sync batched GEMV; above: the cluster split-K wgmma kernel
 constexpr int STEP_SPLITK_MAX_B = 128;    // sequences on the N side of one wgmma tile (BN = 16 / 32 / 64 / 128)
-constexpr int STEP_SPLITK_TILES = 160;   // workspace bound on split * ceil(N / 128); the default budget is one tile per SM, sm_count()
 static StepWs carve_step(const stb_model* m, int B, void* ws) {
     const bool lo = m->prec == STB_PREC_FP16X3;
     const size_t d = m->dims.n_text_state;
@@ -437,7 +424,6 @@ static StepWs carve_step(const stb_model* m, int B, void* ws) {
     w.hid = take_split(c, (size_t)B * 4 * d, lo);
     w.xs = take_split(c, (size_t)B * d, lo);
     w.stats = c.take<float>((size_t)16 * B * 2);
-    w.part = (B > step_gemv_max_b() && B <= STEP_SPLITK_MAX_B) ? c.take<float>((size_t)B * STEP_SPLITK_TILES * 128) : nullptr;
     w.bytes = c.off;
     return w;
 }
@@ -447,11 +433,8 @@ static size_t decode_state_bytes(const stb_model* m, int B, int cache_rows) {
 
 // seq_off (nullable) [B]: first cache row of each sequence; cache_rows: rows per sequence of the K/V caches (>= n_text_ctx
 // when ragged initial tokens are right-aligned, so that the shortest sequence still reaches its own n_text_ctx positions)
-// kv_total / kv_off: the cross K/V block was built for kv_total windows and this step's B sequences are its windows
-// [kv_off, kv_off + B) -- a batch can be stepped as two halves on two streams over ONE block (decode.py: DualStepEngine)
 static int decode_step(stb_model* m, const int32_t* tokens, int B, int32_t* pos, const int32_t* seq_off, int cache_rows,
-                       const void* ckv, int kv_total, int kv_off, void* state, float* logits, long long ld_logits, void* ws,
-                       cudaStream_t st) {
+                       const void* ckv, void* state, float* logits, long long ld_logits, void* ws, cudaStream_t st) {
     const stb_dims& D = m->dims;
     const int d = D.n_text_state, H = D.n_text_head, ctx = cache_rows;
     const void* const(*t)[2] = m->t;
@@ -459,25 +442,20 @@ static int decode_step(stb_model* m, const int32_t* tokens, int B, int32_t* pos,
     const size_t cache = (size_t)B * ctx * d;
     const void* emb_hi = t[STB_T_DEC_TOKEMB][0];
     const void* emb_lo = m->prec == STB_PREC_FP16X3 ? t[STB_T_DEC_TOKEMB][1] : nullptr;
-    // Linear layers of the step, by batch size:
+    // Linear layers of the step, by shape:
     //   B <= 16      : latency-optimised batched GEMV (mma.sync, gemv.cu) -- one launch, weights straight into fragments
-    //   17 .. 128    : SWAPPED wgmma GEMM: the features take the 128-row M side (every weight byte is read by exactly
-    //                  one CTA), the sequences the N side (BN = 32/64/128).  Default: decode_linear.cu -- split-K across a
-    //                  thread-block cluster, partial tiles reduced over distributed shared memory, fused epilogue, ONE
-    //                  launch.  Option decode_splitk_legacy (round 1): the K range cut into `split` slices on the GEMM batch
-    //                  axis, partials [split][B][N] in L2, splitk_finish_kernel adds bias / GELU / residual / LayerNorm
-    //   > 128        : the plain wgmma GEMM (sequences on the M side)
-    const bool use_gemv = B <= step_gemv_max_b(), use_splitk = !use_gemv && B <= STEP_SPLITK_MAX_B;
-    static const int tile_budget = env_int("STB_STEP_SPLIT_TILES", sm_count(), 1, STEP_SPLITK_TILES);
-    const bool legacy_splitk = option(OPT_DECODE_SPLITK_LEGACY) != 0;
+    //   17 .. 128    : SWAPPED wgmma GEMM (decode_linear.cu): the features take the 128-row M side (every weight byte is
+    //                  read by exactly one CTA), the sequences the N side (BN = 32/64/128); split-K across a thread-block
+    //                  cluster, partial tiles reduced over distributed shared memory, fused epilogue, ONE launch.  Needs
+    //                  k % 64 == 0 and n >= 128
+    //   otherwise    : the plain wgmma GEMM (sequences on the M side); with n_text_state % 128 == 0 the only shape the
+    //                  cluster kernel refuses is a vocabulary below 128
+    const bool use_gemv = B <= STEP_GEMV_MAX_B, use_splitk = !use_gemv && B <= STEP_SPLITK_MAX_B;
     const Split none = {nullptr, nullptr};
     // ln_g != nullptr: also produce LayerNorm(out)*ln_g+ln_b into w.ln (only with a residual, out_f32 = w.x)
-    int lin_priority = 0;
-    if (option(OPT_DECODE_LIN_PRIORITY) != 0) {
-        int least = 0, greatest = 0;
-        if (cudaDeviceGetStreamPriorityRange(&least, &greatest) == cudaSuccess) lin_priority = greatest;   // e.g. -5
-    }
-    struct PriorityScope {                                     // the linears (and their fused finish / LayerNorm) only
+    int least = 0, lin_priority = 0;                           // the linears launch at the device's greatest priority (e.g. -5)
+    if (cudaDeviceGetStreamPriorityRange(&least, &lin_priority) != cudaSuccess) lin_priority = 0;
+    struct PriorityScope {                                     // the linears (and their LayerNorm) only
         int saved;
         explicit PriorityScope(int p) : saved(launch_priority()) { launch_priority() = p; }
         ~PriorityScope() { launch_priority() = saved; }
@@ -486,8 +464,7 @@ static int decode_step(stb_model* m, const int32_t* tokens, int B, int32_t* pos,
     // folded weights were supplied for every layer and the width is a whole number of 128-feature tiles.  Only in FP16X3:
     // with one fp16 plane the folded GEMM multiplies the raw, un-centred row, whose rounding error after centring grows
     // as 2^-11 |mean| / std, where the LayerNorm kernels round the normalised row (2^-11)
-    bool fused_ln = option(OPT_DECODE_FUSED_LN) != 0 && m->prec == STB_PREC_FP16X3 && use_splitk && !legacy_splitk &&
-                    d % 128 == 0 && d / 128 <= 16 &&
+    bool fused_ln = option(OPT_DECODE_FUSED_LN) != 0 && m->prec == STB_PREC_FP16X3 && use_splitk && d % 128 == 0 && d / 128 <= 16 &&
                     t[STB_T_DEC_TOKEMB_G][0] != nullptr && t[STB_T_DEC_TOKEMB_FOLD][0] != nullptr;
     for (int l = 0; fused_ln && l < D.n_text_layer; ++l)
         for (int id = STB_L_QKV_WG; id < STB_L_COUNT; ++id)
@@ -499,43 +476,15 @@ static int decode_step(stb_model* m, const int32_t* tokens, int B, int32_t* pos,
                    const float* res, float* out_f32, Split out_split, long long ld, const float* ln_g,
                    const float* ln_b, const DLFuse* fuse = nullptr) -> int {
         PriorityScope prio(lin_priority);
-        if (fuse != nullptr) {                                 // fused route: always the cluster kernel
-            STB_REQUIRE(use_splitk && !legacy_splitk && k % 64 == 0 && n >= 128, "decode_step: folded LayerNorm off the cluster route");
+        const bool cluster = use_splitk && k % 64 == 0 && n >= 128;
+        if (fuse != nullptr) {                                 // folded LayerNorm: always the cluster kernel
+            STB_REQUIRE(cluster, "decode_step: folded LayerNorm off the cluster route");
             return decode_linear(x.hi, x.lo, B, k, w_hi, w_lo, n, bias, act, res, ld, out_f32, out_split.hi, out_split.lo, ld, fuse, st);
         }
         if (use_gemv) {
             STB_TRY(gemv(x.hi, x.lo, B, k, w_hi, w_lo, n, bias, act, res, ld, out_f32, out_split.hi, out_split.lo, ld, st));
-        } else if (use_splitk && !legacy_splitk && k % 64 == 0 && n >= 128) {
-            // one launch: cluster split-K + DSMEM reduction + fused epilogue (decode_linear.cu)
+        } else if (cluster) {
             STB_TRY(decode_linear(x.hi, x.lo, B, k, w_hi, w_lo, n, bias, act, res, ld, out_f32, out_split.hi, out_split.lo, ld, nullptr, st));
-        } else if (use_splitk) {
-            const int mt = cdiv(n, 128), nkb = k / 64;
-            int split = 1;
-            if (k % 64 == 0)
-                for (int sdiv = 1; sdiv <= nkb; ++sdiv)
-                    if (nkb % sdiv == 0 && (long long)mt * sdiv <= tile_budget && mt * sdiv <= STEP_SPLITK_TILES) split = sdiv;
-            const bool direct = split == 1 && bias == nullptr && act == STB_ACT_NONE && res == nullptr && ln_g == nullptr &&
-                                out_split.hi == nullptr;
-            const int ks = k / split;
-            stb_operand a = {w_hi, w_lo, n, ks, (long long)k, 0, (long long)ks};
-            stb_operand b = {x.hi, x.lo, B, ks, (long long)k, 0, (long long)ks};
-            stb_epilogue e;
-            memset(&e, 0, sizeof(e));
-            e.transposed = 1;                                  // D is [feature][sequence]; store [sequence][feature]
-            e.alpha = 1.0f;
-            if (direct) {
-                e.out_f32 = out_f32;
-                e.ld_out = ld;
-                return gemm(a, b, 1, 1, e, st);
-            }
-            STB_REQUIRE((long long)mt * split <= STEP_SPLITK_TILES || split == 1, "decode_step: split-K workspace bound");
-            STB_REQUIRE((size_t)split * B * n <= (size_t)B * STEP_SPLITK_TILES * 128, "decode_step: split-K partials exceed the workspace");
-            e.out_f32 = w.part;
-            e.ld_out = n;
-            e.out_b_stride = (long long)B * n;
-            STB_TRY(gemm(a, b, split, 1, e, st));
-            return splitk_finish(w.part, split, B, n, bias, act, res, ld, out_f32, out_split.hi, out_split.lo, ld, ln_g, ln_b,
-                                 ln_g ? w.ln.hi : nullptr, ln_g ? w.ln.lo : nullptr, st);
         } else {
             stb_epilogue e;
             memset(&e, 0, sizeof(e));
@@ -543,7 +492,7 @@ static int decode_step(stb_model* m, const int32_t* tokens, int B, int32_t* pos,
             e.bias = bias; e.act = act; e.residual = res; e.ld_res = ld; e.alpha = 1.0f;
             STB_TRY(linear(m, x, B, k, w_hi, w_lo, n, e, st));
         }
-        if (ln_g != nullptr)                                   // paths without the fused finish: standalone LayerNorm
+        if (ln_g != nullptr)
             STB_TRY(layernorm(out_f32, B, n, ln_g, ln_b, w.ln.hi, w.ln.lo, nullptr, st));
         return STB_OK;
     };
@@ -580,9 +529,7 @@ static int decode_step(stb_model* m, const int32_t* tokens, int B, int32_t* pos,
             STB_TRY(lin(w.xs, d, whi, wlo, d, cb, STB_ACT_NONE, nullptr, w.q, none, d, nullptr, nullptr, &f));
             Split Kx, vTx;
             CrossDecodeKV Vd;
-            cross_ptrs(m, kv_total, ckv, l, Kx, vTx, &Vd);
-            Vd.k_hi += (size_t)kv_off * H * STB_N_AUDIO_CTX * 64;
-            Vd.v_hi += (size_t)kv_off * H * STB_N_AUDIO_CTX * 64;
+            cross_ptrs(m, B, ckv, l, Kx, vTx, &Vd);
             STB_TRY(decode_attn_cross(w.q, Vd, B, H, d, w.xpart, w.tickets, w.attn.hi, w.attn.lo, nullptr, st));
             STB_TRY(lin(w.attn, d, W_HI(L, STB_L_COUT_W), W_LO(L, STB_L_COUT_W), d, W_F32(L, STB_L_COUT_B), STB_ACT_NONE, w.x,
                         w.x, w.xs, d, nullptr, nullptr, &prod));
@@ -619,9 +566,7 @@ static int decode_step(stb_model* m, const int32_t* tokens, int B, int32_t* pos,
                     none, d, nullptr, nullptr));
         Split Kx, vTx;
         CrossDecodeKV Vd;
-        cross_ptrs(m, kv_total, ckv, l, Kx, vTx, &Vd);
-        Vd.k_hi += (size_t)kv_off * H * STB_N_AUDIO_CTX * 64;
-        Vd.v_hi += (size_t)kv_off * H * STB_N_AUDIO_CTX * 64;
+        cross_ptrs(m, B, ckv, l, Kx, vTx, &Vd);
         STB_TRY(decode_attn_cross(w.q, Vd, B, H, d, w.xpart, w.tickets, w.attn.hi, w.attn.lo, nullptr, st));
         STB_TRY(lin(w.attn, d, W_HI(L, STB_L_COUT_W), W_LO(L, STB_L_COUT_W), d, W_F32(L, STB_L_COUT_B), STB_ACT_NONE, w.x,
                     w.x, none, d, W_F32(L, STB_L_MLP_LN_G), W_F32(L, STB_L_MLP_LN_B)));
@@ -766,8 +711,8 @@ extern "C" size_t stb_decode_state_bytes_rows(const stb_model* m, int B, int cac
 extern "C" size_t stb_decode_ws_bytes(const stb_model* m, int B) { return m ? stb::carve_step(m, B, nullptr).bytes : 0; }
 
 extern "C" int stb_decode_step_ragged(stb_model* m, const int32_t* tokens_in, int B, int32_t* pos, const int32_t* seq_off,
-                                      int cache_rows, const void* cross_kv, int kv_total, int kv_off, void* state,
-                                      float* logits_out, long long ld_logits, void* ws, size_t ws_bytes, void* stream) {
+                                      int cache_rows, const void* cross_kv, void* state, float* logits_out, long long ld_logits,
+                                      void* ws, size_t ws_bytes, void* stream) {
     STB_REQUIRE(m && tokens_in && pos && cross_kv && state && logits_out && ws && B >= 1, "stb_decode_step: bad arguments");
     STB_REQUIRE(ld_logits >= m->dims.n_vocab && ld_logits % 4 == 0, "stb_decode_step: ld_logits must be >= n_vocab and a multiple of 4");
     STB_REQUIRE(m->dims.n_text_ctx <= 448, "stb_decode_step: n_text_ctx > 448 unsupported");
@@ -775,16 +720,13 @@ extern "C" int stb_decode_step_ragged(stb_model* m, const int32_t* tokens_in, in
                 "stb_decode_step: cache_rows must be in [n_text_ctx, 2 n_text_ctx]");
     STB_TRY(check_weights(m, false, true));
     STB_REQUIRE(ws_bytes >= stb_decode_ws_bytes(m, B), "stb_decode_step: workspace too small");
-    if (kv_total <= 0) { kv_total = B; kv_off = 0; }
-    STB_REQUIRE(kv_off >= 0 && kv_off + B <= kv_total, "stb_decode_step: windows [%d, %d) outside the cross K/V block of %d", kv_off,
-                kv_off + B, kv_total);
-    return stb::decode_step(m, tokens_in, B, pos, seq_off, cache_rows, cross_kv, kv_total, kv_off, state, logits_out, ld_logits, ws,
+    return stb::decode_step(m, tokens_in, B, pos, seq_off, cache_rows, cross_kv, state, logits_out, ld_logits, ws,
                             (cudaStream_t)stream);
 }
 
 extern "C" int stb_decode_step(stb_model* m, const int32_t* tokens_in, int B, int32_t* pos, const void* cross_kv, void* state,
                                float* logits_out, long long ld_logits, void* ws, size_t ws_bytes, void* stream) {
     STB_REQUIRE(m, "stb_decode_step: bad arguments");
-    return stb_decode_step_ragged(m, tokens_in, B, pos, nullptr, m->dims.n_text_ctx, cross_kv, B, 0, state, logits_out, ld_logits,
-                                  ws, ws_bytes, stream);
+    return stb_decode_step_ragged(m, tokens_in, B, pos, nullptr, m->dims.n_text_ctx, cross_kv, state, logits_out, ld_logits, ws,
+                                  ws_bytes, stream);
 }

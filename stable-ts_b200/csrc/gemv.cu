@@ -1,6 +1,6 @@
 // Decode-step linear layers, small batches (the engine uses this kernel for B <= 16 sequences; up to 4 groups of 16 rows per
 // CTA share the register-resident weights, so B <= 64 works): out[b][n] = epi( sum_k W[n][k] * x[b][k] ).
-// Larger batches run as a swapped split-K wgmma GEMM (engine.cu) finished by splitk_finish_kernel below.
+// Larger batches run on the cluster split-K wgmma kernel of decode_linear.cu.
 //
 // With M = B <= 16 rows every weight byte is used once: the op is a batched GEMV bound by HBM (d*d*4 B of weights in
 // parity mode), and its enemy is LATENCY, not FLOPs: a 6.5 MB matrix is 1 us of HBM time.  Design:
@@ -156,131 +156,6 @@ gemv_mma_kernel(const __half* __restrict__ x_hi, const __half* __restrict__ x_lo
             }
         }
     }
-}
-
-// ---------------------------------------------------------------------------------------------------------
-// Finish of a split-K decode linear (17..64 sequences run as a SWAPPED wgmma GEMM, engine.cu: features on the
-// 128-row M side, sequences on the N side, the K range cut into `split` slices on the GEMM batch axis):
-//   v[b][n]  = act( sum_z P[z][b][n] + bias[n] ) + res[b][n]          -> out_f32 and/or split planes
-//   ln[b][n] = LayerNorm(v[b][:])[n] * gamma[n] + beta[n]             -> split planes          (optional, N <= 2048)
-// One CTA per sequence, 256 threads, float4 columns; the partials are L2-resident (written a few us earlier).  The fused
-// LayerNorm (whisper.model.LayerNorm: two-pass fp32 statistics, eps 1e-5) is the one that FOLLOWS a residual linear in
-// the decoder block, so the residual stream makes one trip instead of three.
-// ---------------------------------------------------------------------------------------------------------
-constexpr int SK_THREADS = 256;
-constexpr int SK_LNV = 2;                    // float4 per thread kept for the fused LayerNorm (N <= 2048)
-
-__device__ __forceinline__ float block_sum(float v, float* red) {
-    v = warp_sum(v);
-    __syncthreads();                         // red[] may still be read from the previous reduction
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-    __syncthreads();
-    float t = 0.f;
-#pragma unroll
-    for (int i = 0; i < SK_THREADS / 32; ++i) t += red[i];
-    return t;
-}
-
-__global__ void __launch_bounds__(SK_THREADS)
-splitk_finish_kernel(const float* __restrict__ P, int split, int B, int N, const float* __restrict__ bias, int act,
-                     const float* res, long long ld_res, float* out_f32, __half* __restrict__ out_hi,
-                     __half* __restrict__ out_lo, long long ld_out, const float* __restrict__ ln_g,
-                     const float* __restrict__ ln_b, __half* __restrict__ ln_hi, __half* __restrict__ ln_lo) {
-    __shared__ float red[SK_THREADS / 32];
-    pdl_trigger();
-    pdl_wait();
-    const int row = blockIdx.x;
-    const int nv = N >> 2;
-    const long long zs = (long long)B * N;
-    const float* p0 = P + (long long)row * N;
-    const bool do_ln = ln_g != nullptr;
-    float4 keep[SK_LNV];
-    float s = 0.f;
-#pragma unroll 1
-    for (int it = 0, c4 = threadIdx.x; c4 < nv; c4 += SK_THREADS, ++it) {
-        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-        int z = 0;
-        for (; z + 4 <= split; z += 4) {     // 4 independent loads in flight
-            const float4 a = *reinterpret_cast<const float4*>(p0 + (long long)z * zs + c4 * 4);
-            const float4 b = *reinterpret_cast<const float4*>(p0 + (long long)(z + 1) * zs + c4 * 4);
-            const float4 c = *reinterpret_cast<const float4*>(p0 + (long long)(z + 2) * zs + c4 * 4);
-            const float4 e = *reinterpret_cast<const float4*>(p0 + (long long)(z + 3) * zs + c4 * 4);
-            v.x += (a.x + b.x) + (c.x + e.x);
-            v.y += (a.y + b.y) + (c.y + e.y);
-            v.z += (a.z + b.z) + (c.z + e.z);
-            v.w += (a.w + b.w) + (c.w + e.w);
-        }
-        for (; z < split; ++z) {
-            const float4 a = *reinterpret_cast<const float4*>(p0 + (long long)z * zs + c4 * 4);
-            v.x += a.x; v.y += a.y; v.z += a.z; v.w += a.w;
-        }
-        if (bias != nullptr) {
-            const float4 bv = __ldg(reinterpret_cast<const float4*>(bias) + c4);
-            v.x += bv.x; v.y += bv.y; v.z += bv.z; v.w += bv.w;
-        }
-        if (act == STB_ACT_GELU) {
-            v.x = gelu_erf(v.x); v.y = gelu_erf(v.y); v.z = gelu_erf(v.z); v.w = gelu_erf(v.w);
-        }
-        if (res != nullptr) {
-            const float4 rv = *reinterpret_cast<const float4*>(res + (long long)row * ld_res + c4 * 4);
-            v.x += rv.x; v.y += rv.y; v.z += rv.z; v.w += rv.w;
-        }
-        const long long o = (long long)row * ld_out + c4 * 4;
-        if (out_f32 != nullptr) *reinterpret_cast<float4*>(out_f32 + o) = v;
-        if (out_hi != nullptr) {
-            __half h[4], l[4];
-            split_f16(v.x, h[0], l[0]); split_f16(v.y, h[1], l[1]);
-            split_f16(v.z, h[2], l[2]); split_f16(v.w, h[3], l[3]);
-            *reinterpret_cast<uint2*>(out_hi + o) = *reinterpret_cast<uint2*>(h);
-            if (out_lo != nullptr) *reinterpret_cast<uint2*>(out_lo + o) = *reinterpret_cast<uint2*>(l);
-        }
-        if (do_ln && it < SK_LNV) {
-            keep[it] = v;
-            s += (v.x + v.y) + (v.z + v.w);
-        }
-    }
-    if (!do_ln) return;                      // uniform
-    const float mean = block_sum(s, red) / (float)N;
-    float q = 0.f;
-#pragma unroll
-    for (int it = 0; it < SK_LNV; ++it)
-        if (threadIdx.x + it * SK_THREADS < nv) {
-            const float a = keep[it].x - mean, b = keep[it].y - mean, c = keep[it].z - mean, e = keep[it].w - mean;
-            q += (a * a + b * b) + (c * c + e * e);
-        }
-    const float rstd = 1.0f / sqrtf(block_sum(q, red) / (float)N + 1e-5f);
-#pragma unroll
-    for (int it = 0; it < SK_LNV; ++it) {
-        const int c4 = threadIdx.x + it * SK_THREADS;
-        if (c4 < nv) {
-            const float4 g = __ldg(reinterpret_cast<const float4*>(ln_g) + c4);
-            const float4 bb = __ldg(reinterpret_cast<const float4*>(ln_b) + c4);
-            float4 y;
-            y.x = (keep[it].x - mean) * rstd * g.x + bb.x;
-            y.y = (keep[it].y - mean) * rstd * g.y + bb.y;
-            y.z = (keep[it].z - mean) * rstd * g.z + bb.z;
-            y.w = (keep[it].w - mean) * rstd * g.w + bb.w;
-            __half h[4], l[4];
-            split_f16(y.x, h[0], l[0]); split_f16(y.y, h[1], l[1]);
-            split_f16(y.z, h[2], l[2]); split_f16(y.w, h[3], l[3]);
-            const long long o = (long long)row * N + c4 * 4;
-            *reinterpret_cast<uint2*>(ln_hi + o) = *reinterpret_cast<uint2*>(h);
-            if (ln_lo != nullptr) *reinterpret_cast<uint2*>(ln_lo + o) = *reinterpret_cast<uint2*>(l);
-        }
-    }
-}
-
-int splitk_finish(const float* P, int split, int B, int N, const float* bias, int act, const float* res, long long ld_res,
-                  float* out_f32, void* out_hi, void* out_lo, long long ld_out, const float* ln_g, const float* ln_b,
-                  void* ln_hi, void* ln_lo, cudaStream_t st) {
-    STB_REQUIRE(N % 4 == 0 && ld_out % 4 == 0 && (res == nullptr || ld_res % 4 == 0), "splitk_finish: N, ld must be multiples of 4");
-    STB_REQUIRE(ln_g == nullptr || (N <= 4 * SK_LNV * SK_THREADS && ln_b && ln_hi), "splitk_finish: fused LayerNorm needs N <= %d",
-                4 * SK_LNV * SK_THREADS);
-    ProfScope ps("splitk_finish", st, (double)split * B * N * 4.0 + (double)B * N * 8.0);
-    STB_CUDA_OK(launch_pdl(splitk_finish_kernel, dim3(B), dim3(SK_THREADS), 0, st, P, split, B, N, bias, act, res, ld_res,
-                           out_f32, (__half*)out_hi, (__half*)out_lo, ld_out, ln_g, ln_b, (__half*)ln_hi, (__half*)ln_lo));
-    STB_LAUNCH_OK();
-    return STB_OK;
 }
 
 // x split [B][K] (row pitch K), W split [N][K]; out = act(W x + bias) + res as fp32 and/or split planes.

@@ -51,9 +51,6 @@ int v_headmajor(const __half* vT_hi, int BH, int T, int Tp, __half* v_hi, cudaSt
 int gemv(const void* x_hi, const void* x_lo, int B, int K, const void* w_hi, const void* w_lo, int N, const float* bias,
          int act, const float* res, long long ld_res, float* out_f32, void* out_hi, void* out_lo, long long ld_out,
          cudaStream_t st);
-int splitk_finish(const float* P, int split, int B, int N, const float* bias, int act, const float* res, long long ld_res,
-                  float* out_f32, void* out_hi, void* out_lo, long long ld_out, const float* ln_g, const float* ln_b,
-                  void* ln_hi, void* ln_lo, cudaStream_t st);
 // one Linear of the decode step in one launch: swapped wgmma GEMM, split-K across a thread-block cluster, partial tiles
 // reduced over distributed shared memory, fused bias / GELU / residual epilogue (decode_linear.cu)
 // fuse (nullable): LayerNorm folded into the Linear -- stats_in [tiles_in][B][2] partial (sum, sum of squares about the

@@ -60,14 +60,6 @@ bool pdl_enabled(int kind) {
 
 struct OptDef { const char* name; const char* env; int dflt; };
 static const OptDef g_opt_defs[OPT_COUNT] = {
-    // 1: decode-step linears as round 1 ran them (swapped split-K GEMM with partials in L2 + finish kernel) instead of the
-    // cluster kernel of decode_linear.cu -- kept for A/B timing of the two paths on the same box
-    {"decode_splitk_legacy", "STB_DECODE_SPLITK_LEGACY", 0},
-    // 1: the decode step launches its linear layers with the device's greatest launch priority (matters only when two
-    // half-batches are stepped concurrently on two streams)
-    {"decode_lin_priority", "STB_DECODE_LIN_PRIORITY", 1},
-    // 1: decode-step cross-attention on the warp-level tensor cores (ldmatrix + mma.sync over TMA-swizzled K / V tiles)
-    {"xattn_tc", "STB_XATTN_TC", 1},
     // 1: the decode step folds every LayerNorm into the Linear that follows it (W diag(g) planes + row statistics from the
     // producer's epilogue); needs the optional STB_L_*_WG / *_FOLD tensors, else the step runs its LayerNorm kernels.
     // FP16X3 models only: an FP16 model's step ignores it
@@ -137,7 +129,7 @@ extern "C" int stb_axpby(float* y, const float* x, float a, float b, long long n
 }
 
 extern "C" const char* stb_last_error(void) { return stb::get_error(); }
-extern "C" int stb_abi_version(void) { return 3; }
+extern "C" int stb_abi_version(void) { return 4; }
 extern "C" int stb_set_option(const char* name, int value) {
     STB_REQUIRE(name, "stb_set_option: null name");
     stb::opt_init();

@@ -20,21 +20,6 @@ from . import _lib as L
 from .model import B200Whisper
 
 CHUNK_LENGTH = 30
-DUAL_MIN_BATCH = 32          # below this a step is pure launch latency and two chains only add launches
-
-
-def dual_streams() -> int:
-    """Number of concurrent chains a large batch is stepped as (``DualStepEngine``): STB_DECODE_DUAL = 0 / 1 (default: one
-    chain, one stream), 2 (two halves on two streams), 3, ...  A linear CTA owns its SM's shared memory, so it
-    cannot share an SM with the other chain's attention CTAs and the chains serialise at kernel granularity while every kernel
-    gets smaller; not measured on an H100.  Kept as an opt-in (parity-tested) experiment."""
-    import os
-    v = os.environ.get("STB_DECODE_DUAL", "0")
-    try:
-        n = int(v)
-    except ValueError:
-        n = 0 if v in ("", "false", "False") else 2
-    return n if n >= 2 else 0
 
 
 @dataclass
@@ -91,20 +76,17 @@ class StepEngine:
     """Device state of a batch of B decoding sequences + the two launch sequences of one step."""
 
     def __init__(self, model: B200Whisper, B: int, table_rows: int, reuse_buffers: bool = False,
-                 seq_off: Optional[torch.Tensor] = None, cache_rows: Optional[int] = None, kv_total: int = 0, kv_off: int = 0,
-                 tag: str = ""):
+                 seq_off: Optional[torch.Tensor] = None, cache_rows: Optional[int] = None):
         self.m, self.B, self.rows = model, B, table_rows
         dev, lib, V = model.device, model._lib, model.dims.n_vocab
         self.ldv = (V + 7) // 8 * 8
         # ragged initial tokens: per-sequence first cache row (int32 [B], device) and the rows per sequence of the caches
         self.seq_off = seq_off
         self.cache_rows = int(cache_rows or model.dims.n_text_ctx)
-        # these B sequences are windows [kv_off, kv_off + B) of a cross K/V block built for kv_total windows (0: the block's own)
-        self.kv_total, self.kv_off = int(kv_total), int(kv_off)
         state_bytes = lib.stb_decode_state_bytes_rows(model._h, B, self.cache_rows)
         if reuse_buffers:      # model-owned: the self-attention K/V cache (rows beyond `pos` are never read) and the workspace
-            self.state = model._buf("decode_state" + tag, state_bytes)
-            self.ws = model._buf("decode_ws" + tag, lib.stb_decode_ws_bytes(model._h, B))
+            self.state = model._buf("decode_state", state_bytes)
+            self.ws = model._buf("decode_ws", lib.stb_decode_ws_bytes(model._h, B))
             self.ws.zero_()                                                                          # tickets start at 0
         else:
             self.state = torch.zeros(state_bytes, dtype=torch.uint8, device=dev)
@@ -131,8 +113,8 @@ class StepEngine:
         """decoder step for tokens [B] int32 (device) -> self.logits; pos += 1"""
         m = self.m
         L.check(m._lib.stb_decode_step_ragged(m._h, L.ptr(tokens), self.B, L.ptr(self.pos), L.ptr(self.seq_off),
-                                              self.cache_rows, L.ptr(ckv), self.kv_total, self.kv_off, L.ptr(self.state),
-                                              L.ptr(self.logits), self.ldv, L.ptr(self.ws), self.ws.numel(), L.stream_ptr()))
+                                              self.cache_rows, L.ptr(ckv), L.ptr(self.state), L.ptr(self.logits), self.ldv,
+                                              L.ptr(self.ws), self.ws.numel(), L.stream_ptr()))
 
     def step(self, ckv, *sample_args):
         """one decoding step: pick the next token from the current logits, then run the decoder on it"""
@@ -147,91 +129,6 @@ class StepEngine:
                                   int(max_initial_ts), int(apply_ts_rules), L.ptr(self.forced),
                                   L.ptr(self.seq), L.ptr(self.next), L.ptr(self.tok_table), L.ptr(self.arg_table),
                                   self.rows, float(self.temperature), L.ptr(self.uniform), L.ptr(self.cap), L.stream_ptr()))
-
-
-class DualStepEngine:
-    """The batch stepped as TWO halves on two streams over one cross K/V block (same interface as ``StepEngine``).
-
-    A decode step is a chain of ~11 dependent launches per layer: the linear layers are latency-bound (a few MB of weights
-    each on 80-120 SMs), the cross-attention is HBM-bound.  Two independent chains interleave: while one half streams its
-    cross K/V, the other half's linears run -- launched at the device's greatest priority (``decode_lin_priority``), so the
-    block scheduler serves a pending linear before the other half's remaining attention CTAs.  Both halves are captured into
-    ONE graph (fork / join per step).  The weights are read once per half (12 GB instead of 6 GB per step at large-v3, against
-    30 GB of cross K/V)."""
-
-    def __init__(self, model: B200Whisper, B: int, table_rows: int, reuse_buffers: bool = False,
-                 seq_off: Optional[torch.Tensor] = None, cache_rows: Optional[int] = None, n_parts: Optional[int] = None):
-        n_parts = max(2, min(int(n_parts or dual_streams()), B))
-        self.m, self.B, self.rows = model, B, table_rows
-        cuts = [(B * i) // n_parts for i in range(n_parts + 1)]
-        self.parts = list(zip(cuts[:-1], cuts[1:]))
-        self.engs = [StepEngine(model, hi - lo, table_rows, reuse_buffers=reuse_buffers,
-                                seq_off=None if seq_off is None else seq_off[lo:hi].contiguous(), cache_rows=cache_rows,
-                                kv_total=B, kv_off=lo, tag=f"_{i}") for i, (lo, hi) in enumerate(self.parts)]
-        self.ldv = self.engs[0].ldv
-        self.side = [torch.cuda.Stream(device=model.device) for _ in self.parts[1:]]
-        self.graph, self.graph_nodes = None, 0
-
-    def reset(self):
-        for e in self.engs:
-            e.reset()
-
-    def _split_cols(self, t):
-        return [None if t is None else t[..., lo:hi].contiguous() for lo, hi in self.parts]
-
-    cap = property(lambda self: self.engs[0].cap)
-    temperature = property(lambda self: self.engs[0].temperature)
-    uniform = property(lambda self: self.engs[0].uniform)
-    forced = property(lambda self: self.engs[0].forced)
-
-    @cap.setter
-    def cap(self, t):
-        for e, v in zip(self.engs, self._split_cols(t)):
-            e.cap = v
-
-    @temperature.setter
-    def temperature(self, t):
-        for e in self.engs:
-            e.temperature = t
-
-    @uniform.setter
-    def uniform(self, t):
-        for e, v in zip(self.engs, self._split_cols(t)):
-            e.uniform = v
-
-    @forced.setter
-    def forced(self, t):
-        for e, v in zip(self.engs, self._split_cols(t)):
-            e.forced = v
-
-    logits = property(lambda self: torch.cat([e.logits for e in self.engs]))
-    seq = property(lambda self: torch.cat([e.seq for e in self.engs]))
-    tok_table = property(lambda self: torch.cat([e.tok_table for e in self.engs], dim=1))
-    arg_table = property(lambda self: torch.cat([e.arg_table for e in self.engs], dim=1))
-
-    def _part_args(self, i, tk, suppress, first_mask, ts_mask, max_initial_ts, apply_ts_rules):
-        lo, hi = self.parts[i]
-        if ts_mask is not None and ts_mask.ndim == 2:
-            ts_mask = ts_mask[lo:hi]                       # contiguous rows of the [B, 1501] mask
-        return tk, suppress, first_mask, ts_mask, max_initial_ts, apply_ts_rules
-
-    def feed(self, tokens: torch.Tensor, ckv: torch.Tensor):
-        for e, (lo, hi) in zip(self.engs, self.parts):
-            e.feed(tokens[lo:hi], ckv)
-
-    def sample(self, *sample_args):
-        for i, e in enumerate(self.engs):
-            e.sample(*self._part_args(i, *sample_args))
-
-    def step(self, ckv, *sample_args):
-        cur = torch.cuda.current_stream()
-        for i, st in enumerate(self.side, start=1):         # fork
-            st.wait_stream(cur)
-            with torch.cuda.stream(st):
-                self.engs[i].step(ckv, *self._part_args(i, *sample_args))
-        self.engs[0].step(ckv, *self._part_args(0, *sample_args))
-        for st in self.side:                                # join
-            cur.wait_stream(st)
 
 
 def enc_select(enc: dict, idx: Sequence[int]) -> dict:
@@ -326,9 +223,7 @@ def _decode_windows(model: B200Whisper, tokenizer, enc: dict, options: Optional[
     steps = max(min(steps, max(caps)), 0)
     seq_off = torch.tensor([max_init - n for n in lens], dtype=torch.int32, device=dev) if ragged else None
     # (tests/standin.py swaps the engine for a CPU one built on the oracle to pin this host logic without a GPU)
-    engine_cls = getattr(model, "step_engine_cls", None)
-    if engine_cls is None:
-        engine_cls = DualStepEngine if (dual_streams() and B >= DUAL_MIN_BATCH and not return_step_logits) else StepEngine
+    engine_cls = getattr(model, "step_engine_cls", None) or StepEngine
     eng = engine_cls(model, B, max(steps, 1), reuse_buffers=reuse_buffers, seq_off=seq_off,
                      cache_rows=n_ctx + (max_init - min_init))
     eng.reset()
@@ -408,7 +303,7 @@ def _decode_windows(model: B200Whisper, tokenizer, enc: dict, options: Optional[
         elif return_step_logits:
             eng.sample(tokenizer, sup, first, tsm, max_init_ts, apply_rules)
             step_logits.append(eng.logits[:, :V].clone())
-            eng.feed(eng.next, ckv)                    # (plain StepEngine: the dual engine is not used with step logits)
+            eng.feed(eng.next, ckv)
         elif use_graph and done_steps >= 1:
             if eng.graph is None:
                 torch.cuda.synchronize()

@@ -50,24 +50,26 @@ def test_product_path_fails_loudly_without_cuda():
         B200Whisper(None, {}, device="cuda")
 
 
-def test_option_switches_and_error_reporting_without_a_gpu():
-    """stb_set_option / stb_get_option / stb_last_error work without a device: defaults of the kernel-variant switches, unknown
-    names are an error with a message (include/stablets_b200.h)."""
+def test_option_switch_and_error_reporting_without_a_gpu():
+    """stb_set_option / stb_get_option / stb_last_error work without a device: defaults of the kernel-variant switch, unknown
+    names (among them the retired "xattn_tc", "decode_splitk_legacy" and "decode_lin_priority") read as -1 and are an error
+    with a message (include/stablets_b200.h)."""
     from stable_ts_b200 import _lib as L
     lib = L.lib()
-    assert lib.stb_abi_version() >= 3
-    assert L.get_option("xattn_tc") in (0, 1) and L.get_option("decode_splitk_legacy") in (0, 1)
-    assert L.get_option("decode_fused_ln") in (0, 1) and L.get_option("no_such_option") == -1
-    old = L.get_option("decode_splitk_legacy")
-    L.set_option("decode_splitk_legacy", 1 - old)
-    assert L.get_option("decode_splitk_legacy") == 1 - old
-    L.set_option("decode_splitk_legacy", old)
-    try:
-        L.set_option("no_such_option", 1)
-    except L.StbError as e:
-        assert "no_such_option" in str(e)
-    else:
-        raise AssertionError("unknown option accepted")
+    assert lib.stb_abi_version() >= 4
+    assert L.get_option("decode_fused_ln") in (0, 1)
+    old = L.get_option("decode_fused_ln")
+    L.set_option("decode_fused_ln", 1 - old)
+    assert L.get_option("decode_fused_ln") == 1 - old
+    L.set_option("decode_fused_ln", old)
+    for name in ("no_such_option", "xattn_tc", "decode_splitk_legacy", "decode_lin_priority"):
+        assert L.get_option(name) == -1
+        try:
+            L.set_option(name, 1)
+        except L.StbError as e:
+            assert name in str(e)
+        else:
+            raise AssertionError(f"unknown option {name!r} accepted")
     # argument validation happens before any CUDA call
     assert lib.stb_decode_state_bytes(None, 4) == 0 and lib.stb_decode_ws_bytes(None, 4) == 0
     assert lib.stb_axpby(None, None, 1.0, 0.0, 8, None) != 0 and b"stb_axpby" in lib.stb_last_error()

@@ -163,9 +163,9 @@ def test_decode_batch_above_64_takes_tcgen05_step():
 
 
 def test_large_width_step_paths_agree():
-    """large-v3 widths (d = 1280, 20 heads, 51866 tokens; 1 encoder + 2 decoder layers): the three decode-step linear
-    paths -- mma.sync GEMV (B = 2), swapped split-K wgmma GEMM + fused finish/LayerNorm (B = 20 and 50: BN = 32 / 64,
-    K = 1280 and 5120 splits, direct vocabulary projection) -- must produce the same step logits and tokens."""
+    """large-v3 widths (d = 1280, 20 heads, 51866 tokens; 1 encoder + 2 decoder layers): the two decode-step linear
+    routes -- mma.sync GEMV (B = 2) and the cluster split-K wgmma kernel (B = 20 and 50: BN = 32 / 64, K = 1280 and 5120,
+    vocabulary projection) -- must produce the same step logits and tokens."""
     if not torch.cuda.is_available():
         pytest.skip("no CUDA device")
     from oracle import stable_path as SP
@@ -200,77 +200,68 @@ def test_large_width_step_paths_agree():
             assert rg[j].tokens == r2[j % 2].tokens
 
 
-@pytest.mark.parametrize("chains", [2, 3])
-def test_batch_stepped_as_concurrent_chains_matches_one_chain(chains, monkeypatch):
-    """DualStepEngine (STB_DECODE_DUAL): the batch as 2 / 3 chains on separate streams over ONE cross K/V block
-    (stb_decode_step_ragged kv_total / kv_off), captured into one graph -- same tokens and log-probs as the single chain."""
+def test_cross_attention_step_logits_match_float64():
+    """The decode-step cross-attention (mma.sync over TMA-swizzled fp16 K / V tiles) at large-v3 widths (d = 1280, 20 heads,
+    51866 tokens; 1 encoder + 2 decoder layers), behind the GEMV (B = 3) and the cluster (B = 42) linears, with a window whose
+    tail is silence: step logits of a forced token script against the oracle's decode in float64, fed this library's own
+    encoder output so that only the decode step is measured.  Then graph replay against eager stepping, and a free-running
+    tiny.en decode against the CPU oracle."""
     if not torch.cuda.is_available():
         pytest.skip("no CUDA device")
+    import copy
+    import torch.nn.functional as F
     from oracle import stable_path as SP
+    from oracle.whisper_ref import model as WM
     from oracle.whisper_ref.model import ModelDimensions
-    from stable_ts_b200.decode import DecodingOptions, decode_windows
-    dims = ModelDimensions(n_mels=80, n_audio_ctx=1500, n_audio_state=384, n_audio_head=6, n_audio_layer=2, n_vocab=51864,
-                           n_text_ctx=448, n_text_state=384, n_text_head=6, n_text_layer=3)
-    W, model, gm, tk = _mk(dims, 23)
-    audios = torch.stack([SP.synth_audio(480000, seed=300 + i) for i in range(7)]).repeat(6, 1)       # 42 windows
-    enc = gm.encode(gm.log_mel(audios.cuda()))
-    opt = DecodingOptions(sample_len=12)
-    monkeypatch.setenv("STB_DECODE_DUAL", "0")
-    one, _ = decode_windows(gm, tk, enc, opt)
-    monkeypatch.setenv("STB_DECODE_DUAL", str(chains))
-    many, ex = decode_windows(gm, tk, enc, opt)
-    for a, b in zip(one, many):
-        assert a.tokens == b.tokens and abs(a.avg_logprob - b.avg_logprob) < 1e-5
-        assert abs(a.no_speech_prob - b.no_speech_prob) <= 1e-6 + 1e-4 * a.no_speech_prob
-
-
-def test_cross_attention_tensor_core_variant():
-    """Option "xattn_tc": the decode-step cross-attention on mma.sync over TMA-swizzled tiles must give the step logits of the
-    scalar kernel (both fp32-grade in q, fp16 K / V) and the oracle's tokens."""
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from oracle import stable_path as SP
-    from oracle.whisper_ref.model import ModelDimensions
-    from stable_ts_b200 import _lib as L
     from stable_ts_b200.decode import DecodingOptions, decode_windows
     dims = ModelDimensions(n_mels=128, n_audio_ctx=1500, n_audio_state=1280, n_audio_head=20, n_audio_layer=1, n_vocab=51866,
                            n_text_ctx=448, n_text_state=1280, n_text_head=20, n_text_layer=2)
     W, model, gm, tk = _mk(dims, 17)
+    m64 = copy.deepcopy(model).double()
     audios = torch.stack([SP.synth_audio(480000, seed=90 + i) for i in range(3)])
     audios[2, 200000:] = 0                                    # a window whose tail is silence
-    opt = DecodingOptions(sample_len=6)
-    V = dims.n_vocab
-    default = L.get_option("xattn_tc")
-    try:
-        for rep in (1, 14):                                   # B = 3 (GEMV path) and B = 42 (cluster linears)
+    steps = 8
+    script = SP.synth_token_script(steps, tk.eot, seed=11)
+    opt = DecodingOptions(language="en", sample_len=steps)
+    mel = torch.zeros(dims.n_mels, 3000)                      # (not read: the oracle is given the audio features)
+    refs = []                                                 # (float64 encoder output of a window, its step logits)
+    with pytest.MonkeyPatch.context() as mp:
+        # the oracle's LayerNorm computes in fp32 (a guard for fp16 models); in the float64 model it keeps float64
+        mp.setattr(WM.LayerNorm, "forward", lambda self, x: F.layer_norm(x, self.normalized_shape, self.weight, self.bias, self.eps))
+        for rep in (1, 14):                                   # B = 3 (GEMV linears) and B = 42 (cluster linears)
+            B = 3 * rep
             enc = gm.encode(gm.log_mel(audios.repeat(rep, 1).cuda()))
-            L.set_option("xattn_tc", 0)
-            r0, x0 = decode_windows(gm, tk, enc, opt, return_step_logits=True)
-            for variant in (1,):
-                L.set_option("xattn_tc", variant)
-                r1, x1 = decode_windows(gm, tk, enc, opt, return_step_logits=True)
-                worst = 0.0
-                for a, b in zip(x0["step_logits"], x1["step_logits"]):
-                    a, b = a.float().cpu(), b.float().cpu()
-                    fin = a > -1e30
-                    assert torch.equal(fin, b > -1e30)
-                    worst = max(worst, ((a[fin] - b[fin]).abs().max() / a[fin].abs().max()).item())
-                print(f"B={3 * rep}: tensor-core variant {variant} vs scalar cross-attention, worst step-logit rel diff {worst:.2e}")
-                assert worst < 2e-5
-                for a, b in zip(r0, r1):
-                    assert a.tokens == b.tokens
-                rg, _ = decode_windows(gm, tk, enc, opt)      # graph replay with the option on
-                for a, b in zip(r0, rg):
-                    assert a.tokens == b.tokens
-            L.set_option("xattn_tc", default)
-        # against the CPU oracle (tiny.en, free-running greedy)
-        W2, om, gm2, tk2 = _mk("tiny.en", 3)
-        audio = SP.synth_audio(480000, seed=7)
-        ref, _, _ = SP.decode_window(om, _mel(W2, om, audio), language="en", sample_len=16)
-        res, _ = decode_windows(gm2, tk2, gm2.encode(gm2.log_mel(audio.cuda()[None])), DecodingOptions(language="en", sample_len=16))
-        assert res[0].tokens == ref.tokens and abs(res[0].avg_logprob - ref.avg_logprob) < 1e-3
-    finally:
-        L.set_option("xattn_tc", default)
+            _, x = decode_windows(gm, tk, enc, opt, forced_tokens=torch.tensor(script)[:, None].repeat(1, B),
+                                  return_step_logits=True)
+            feats = enc["f32"].view(B, dims.n_audio_ctx, -1).cpu().double()
+            worst = 0.0
+            for j in range(B):
+                ref = next((r for a, r in refs if torch.equal(a, feats[j])), None)
+                if ref is None:
+                    _, _, ex = SP.decode_window(m64, mel, audio_features=feats[j:j + 1], forced_tokens=script,
+                                                return_step_logits=True, sample_len=steps, language="en")
+                    ref = ex["step_logits"]
+                    refs.append((feats[j], ref))
+                assert len(ref) == len(x["step_logits"]) == steps
+                for r, g in zip(ref, x["step_logits"]):
+                    r, g = r.double(), g[j].double().cpu()
+                    fin = r > -1e30
+                    assert torch.equal(fin, g > -1e30)
+                    worst = max(worst, ((g[fin] - r[fin]).abs().max() / r[fin].abs().max()).item())
+            print(f"B={B}: decode step vs float64 oracle, worst step-logit rel err {worst:.2e}")
+            # measured on an NVIDIA H100 80GB HBM3 at 700 W: 9.70e-6 (B = 3) and 1.19e-5 (B = 42) with this kernel, 9.75e-6
+            # and 1.19e-5 with the scalar-lane kernel it replaced; the bound is 1.25x the worst, rounded up
+            assert worst < 2e-5
+            r_eager, _ = decode_windows(gm, tk, enc, opt, use_graph=False)
+            r_graph, _ = decode_windows(gm, tk, enc, opt)     # CUDA-graph replay of the same step
+            for a, b in zip(r_eager, r_graph):
+                assert a.tokens == b.tokens
+    # against the CPU oracle (tiny.en, free-running greedy)
+    W2, om, gm2, tk2 = _mk("tiny.en", 3)
+    audio = SP.synth_audio(480000, seed=7)
+    ref, _, _ = SP.decode_window(om, _mel(W2, om, audio), language="en", sample_len=16)
+    res, _ = decode_windows(gm2, tk2, gm2.encode(gm2.log_mel(audio.cuda()[None])), DecodingOptions(language="en", sample_len=16))
+    assert res[0].tokens == ref.tokens and abs(res[0].avg_logprob - ref.avg_logprob) < 1e-3
 
 
 def test_layernorm_folded_into_the_step_linears():
@@ -310,38 +301,3 @@ def test_layernorm_folded_into_the_step_linears():
                 assert a.tokens == b.tokens
     finally:
         L.set_option("decode_fused_ln", default)
-
-
-def test_splitk_finish_linears_option_matches_cluster_linears():
-    """Option "decode_splitk_legacy": the round-1 route of the decode-step linears (swapped split-K wgmma GEMM with partials in
-    L2 + finish kernel with the fused LayerNorm) against the cluster kernel: same step logits and tokens."""
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from oracle import stable_path as SP
-    from oracle.whisper_ref.model import ModelDimensions
-    from stable_ts_b200 import _lib as L
-    from stable_ts_b200.decode import DecodingOptions, decode_windows
-    dims = ModelDimensions(n_mels=128, n_audio_ctx=1500, n_audio_state=1280, n_audio_head=20, n_audio_layer=1, n_vocab=51866,
-                           n_text_ctx=448, n_text_state=1280, n_text_head=20, n_text_layer=2)
-    W, model, gm, tk = _mk(dims, 31)
-    audios = torch.stack([SP.synth_audio(480000, seed=500 + i) for i in range(3)])
-    enc = gm.encode(gm.log_mel(audios.repeat(14, 1).cuda()))          # B = 42
-    opt = DecodingOptions(sample_len=6)
-    default = L.get_option("decode_splitk_legacy")
-    try:
-        L.set_option("decode_splitk_legacy", 0)
-        r0, x0 = decode_windows(gm, tk, enc, opt, return_step_logits=True)
-        L.set_option("decode_splitk_legacy", 1)
-        r1, x1 = decode_windows(gm, tk, enc, opt, return_step_logits=True)
-        worst = 0.0
-        for a, b in zip(x0["step_logits"], x1["step_logits"]):
-            a, b = a.float().cpu(), b.float().cpu()
-            fin = a > -1e30
-            assert torch.equal(fin, b > -1e30)
-            worst = max(worst, ((a[fin] - b[fin]).abs().max() / a[fin].abs().max()).item())
-        print(f"B=42: split-K + finish vs cluster linears, worst step-logit rel diff {worst:.2e}")
-        assert worst < 2e-5
-        for a, b in zip(r0, r1):
-            assert a.tokens == b.tokens
-    finally:
-        L.set_option("decode_splitk_legacy", default)

@@ -15,7 +15,7 @@ ALLOW = {            # kernel-name substring -> what its early non-coherent load
 }
 # Asynchronous copies (TMA `UTMALDG`, bulk `UBLKCP`) that are issued ahead of the wait ON PURPOSE -- listed with `--all`:
 #   decode_linear_kernel            the WEIGHT tiles of the first ring stages (the activations are loaded after the wait)
-#   decode_cross_attn(_tc)_kernel   the window's cross K / V tiles: written once per window batch by stb_cross_kv, many
+#   decode_cross_attn_tc_kernel     the window's cross K / V tiles: written once per window batch by stb_cross_kv, many
 #                                   kernels earlier on the same stream (every kernel in between waited on its predecessor)
 
 

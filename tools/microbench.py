@@ -43,47 +43,6 @@ def _time(fn, iters, graph=True):
     return e0.elapsed_time(e1) / (iters * reps) * 1e3      # us
 
 
-def bench_splitk(batches=(16, 64), iters=40):
-    """decode-step linear as a SWAPPED split-K wgmma GEMM through stb_gemm: A = W (features on the 128-row M side), B = x
-    (sequences on the N side), the K range cut into `split` slices mapped on the GEMM batch axis; partials [split][B][N]."""
-    import ctypes
-    lib = L.lib()
-    out = []
-    for Bn in batches:
-        for (N, K, split) in ((1280, 1280, 10), (1280, 1280, 5), (3840, 1280, 5), (5120, 1280, 4), (1280, 5120, 16),
-                              (1280, 5120, 8), (51866, 1280, 1)):
-            ks = K // split
-            copies = max(2, int(300e6 // (N * K * 4)) + 1)
-            W = torch.randn(copies, N, K, device="cuda") * 0.05
-            wh = W.half()
-            wl = (W - wh.float()).half()
-            X = torch.randn(Bn, K, device="cuda")
-            xh = X.half()
-            xl = (X - xh.float()).half()
-            P = torch.zeros(split, Bn, N, device="cuda")
-
-            def run(i):
-                c = i % copies
-                a = L.Operand(L.ptr(wh[c]), L.ptr(wl[c]), N, ks, K, 0, ks)
-                b = L.Operand(L.ptr(xh), L.ptr(xl), Bn, ks, K, 0, ks)
-                ep = L.Epilogue()
-                ep.out_f32 = L.ptr(P)
-                ep.ld_out = N
-                ep.out_b_stride = Bn * N
-                ep.transposed = 1
-                ep.alpha = 1.0
-                L.check(lib.stb_gemm(ctypes.byref(a), ctypes.byref(b), split, 1, ctypes.byref(ep), L.stream_ptr()))
-            run(0)
-            torch.cuda.synchronize()
-            ref = X.double() @ W[0].double().T
-            err = ((P.double().sum(0) - ref).abs().max() / ref.abs().max()).item()
-            us = _time(run, iters)
-            out.append(dict(B=Bn, N=N, K=K, split=split, us=round(us, 2), weight_GBps=round(N * K * 4 / us / 1e3, 1), rel_err=err))
-            print(out[-1], flush=True)
-            del W, wh, wl
-    return out
-
-
 def bench_gemv(batches=(16, 64), shapes=((1280, 1280), (3840, 1280), (5120, 1280), (1280, 5120), (51866, 1280)), iters=200):
     lib = L.lib()
     out = []
@@ -129,7 +88,7 @@ def bench_dtw(batches=(16, 64, 148)):
 def bench_step(windows=120, layers=4, s1=24, s2=72):
     """ms per KV-cached decode step of a large-v3-WIDTH model with `layers` decoder layers (cross K/V of 120 windows x 32
     layers would not leave room for A/B runs), from the slope between two forced decodes of s1 and s2 steps (graph replay).
-    Use with STB_DECODE_SPLITK_LEGACY=1 / STB_STEP_* to A/B the decode-step variants:  microbench.py step [windows] [layers]"""
+    Use with STB_DECODE_FUSED_LN=1 to A/B the folded LayerNorm:  microbench.py step [windows] [layers]"""
     import time
     from stable_ts_b200.api import random_state_dict
     from stable_ts_b200.decode import DecodingOptions, decode_windows
@@ -174,5 +133,5 @@ if __name__ == "__main__":
     elif what == "ncu":          # short run for `ncu -k regex:...`: fc1 / fc2 at 64 sequences + one DTW batch
         res = [bench_gemv((64,), ((5120, 1280), (1280, 5120)), iters=4), bench_dtw((16,))]
     else:
-        res = {"gemv": bench_gemv, "dtw": bench_dtw, "splitk": bench_splitk}[what]()
+        res = {"gemv": bench_gemv, "dtw": bench_dtw}[what]()
     print(json.dumps({what: res, "env": {k: v for k, v in os.environ.items() if k.startswith("STB_")}}))
