@@ -314,6 +314,26 @@ STB_API int stb_decode_step_ragged(stb_model* m, const int32_t* tokens_in, int B
                            int cache_rows, const void* cross_kv, void* state, float* logits_out, long long ld_logits,
                            void* ws, size_t ws_bytes, void* stream);
 
+/* The two attention kernels of the decode step on their own, exposed for tests (csrc/decode.cu).  d = 64 H; B and H in
+ *    1..65535.  Outputs: out_f32 fp32 [B][d] and/or split planes out_hi / out_lo fp16 [B][d] (hi = rn(o), lo = rn(o - hi);
+ *    out_lo needs out_hi); at least one of out_f32 / out_hi.
+ * stb_decode_self_attn: one head-sliced attention of the newest token over the fp32 self-attention K/V cache.
+ *    qkv fp32 [B][3d] (q | k | v of the newest token); k_cache, v_cache fp32 [B][cache_rows][d]; pos a DEVICE int32 counter;
+ *    seq_off (nullable) a device int32 [B] of first cache rows (NULL: 0).  The kernel writes the k / v slices of qkv into
+ *    cache row `pos` and writes nothing else of the caches; sequence b then attends rows [min(seq_off[b], pos), pos] with
+ *    weights softmax(q . K[j] / 8), and never reads any other row.  pos < cache_rows is the caller's duty (the host cannot
+ *    read the counter).  qkv and the caches 16-byte aligned.
+ * stb_decode_cross_attn: attention of one query per sequence over the window's 1500 cross K / V rows.
+ *    q fp32 [B][d]; k_hi, v_hi fp16 head-major [B][H][1500][64] (16-byte aligned: TMA sources), the layout
+ *    stb_cross_kv(..., decode_layout = 1) writes.  partial: scratch of B H stb_decode_cross_splits() 66 floats.
+ *    tickets: B H int32 that must be zero before the first call; every call leaves them zero again, so one pair of
+ *    partial / tickets serves any number of calls on one stream. */
+STB_API int stb_decode_self_attn(const float* qkv, float* k_cache, float* v_cache, int B, int H, int cache_rows, const int32_t* pos,
+                                 const int32_t* seq_off, float* out_f32, void* out_hi, void* out_lo, void* stream);
+STB_API int stb_decode_cross_attn(const float* q, const void* k_hi, const void* v_hi, int B, int H, float* partial, int32_t* tickets,
+                                  float* out_f32, void* out_hi, void* out_lo, void* stream);
+STB_API int stb_decode_cross_splits(void);
+
 /* per-sequence sampling state kept on the device */
 typedef struct {
     int32_t n_sampled;   /* tokens sampled so far (0 at sample_begin) */

@@ -88,6 +88,11 @@ _SIGS = {
     "stb_decode_state_bytes_rows": (c_size_t, [c_void_p, c_int, c_int]),
     "stb_decode_step_ragged": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
                                        c_longlong, c_void_p, c_size_t, c_void_p]),
+    "stb_decode_self_attn": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                     c_void_p, c_void_p]),
+    "stb_decode_cross_attn": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                      c_void_p, c_void_p]),
+    "stb_decode_cross_splits": (c_int, []),
     "stb_sample": (c_int, [c_void_p, c_longlong, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                            c_longlong, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_float, c_void_p,
                            c_void_p, c_void_p]),

@@ -658,7 +658,6 @@ int decode_attn_cross(const float* q, const CrossDecodeKV& kv, int B, int H, int
     STB_LAUNCH_OK();
     return STB_OK;
 }
-size_t decode_cross_scratch_bytes(int B, int H) { return (size_t)B * H * XS * 66 * sizeof(float) + (size_t)B * H * sizeof(int) + 256; }
 int decode_cross_splits() { return XS; }
 int v_headmajor(const __half* vT_hi, int BH, int T, int Tp, __half* v_hi, cudaStream_t st) {
     ProfScope ps("v_headmajor", st, (double)BH * T * 64 * 4.0);
@@ -679,3 +678,46 @@ int bump_pos(int32_t* pos, cudaStream_t st) {
     return STB_OK;
 }
 }  // namespace stb
+
+// ---------------------------------------------------------------------------------------------------------
+// test entry points: the two attention kernels of the decode step on their own (include/stablets_b200.h)
+// ---------------------------------------------------------------------------------------------------------
+static bool aligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
+
+extern "C" int stb_decode_self_attn(const float* qkv, float* k_cache, float* v_cache, int B, int H, int cache_rows, const int32_t* pos,
+                                    const int32_t* seq_off, float* out_f32, void* out_hi, void* out_lo, void* stream) {
+    // grid (H, B): B is grid.y
+    STB_REQUIRE(B >= 1 && B <= 65535, "stb_decode_self_attn: B=%d outside 1..65535", B);
+    STB_REQUIRE(H >= 1 && H <= 65535, "stb_decode_self_attn: H=%d outside 1..65535", H);
+    STB_REQUIRE(cache_rows >= 1, "stb_decode_self_attn: cache_rows=%d must be positive", cache_rows);
+    STB_REQUIRE(qkv && k_cache && v_cache && pos, "stb_decode_self_attn: null qkv, cache or pos");
+    STB_REQUIRE(out_f32 || out_hi, "stb_decode_self_attn: no output (out_f32 and out_hi are both null)");
+    STB_REQUIRE(out_lo == nullptr || out_hi != nullptr, "stb_decode_self_attn: out_lo needs out_hi");
+    // qkv and the caches are read as float4
+    STB_REQUIRE(aligned(qkv, 16) && aligned(k_cache, 16) && aligned(v_cache, 16),
+                "stb_decode_self_attn: qkv, k_cache and v_cache must be 16-byte aligned");
+    STB_REQUIRE(aligned(pos, 4) && aligned(seq_off, 4) && aligned(out_f32, 4) && aligned(out_hi, 2) && aligned(out_lo, 2),
+                "stb_decode_self_attn: misaligned pos, seq_off or output");
+    return stb::decode_attn_self(qkv, k_cache, v_cache, B, H, 64 * H, cache_rows, pos, seq_off, (__half*)out_hi, (__half*)out_lo,
+                                 out_f32, (cudaStream_t)stream);
+}
+
+extern "C" int stb_decode_cross_attn(const float* q, const void* k_hi, const void* v_hi, int B, int H, float* partial, int32_t* tickets,
+                                     float* out_f32, void* out_hi, void* out_lo, void* stream) {
+    // grid (splits, H, B); tickets are indexed b * H + h in int
+    STB_REQUIRE(B >= 1 && B <= 65535, "stb_decode_cross_attn: B=%d outside 1..65535", B);
+    STB_REQUIRE(H >= 1 && H <= 65535 && (long long)B * H <= 0x7fffffffLL, "stb_decode_cross_attn: H=%d outside 1..65535 or B*H too large", H);
+    STB_REQUIRE(q && k_hi && v_hi && partial && tickets, "stb_decode_cross_attn: null q, K / V plane, partial or tickets");
+    STB_REQUIRE(out_f32 || out_hi, "stb_decode_cross_attn: no output (out_f32 and out_hi are both null)");
+    STB_REQUIRE(out_lo == nullptr || out_hi != nullptr, "stb_decode_cross_attn: out_lo needs out_hi");
+    // the K / V planes are TMA sources
+    STB_REQUIRE(aligned(k_hi, 16) && aligned(v_hi, 16), "stb_decode_cross_attn: k_hi and v_hi must be 16-byte aligned");
+    STB_REQUIRE(aligned(q, 4) && aligned(partial, 4) && aligned(tickets, 4) && aligned(out_f32, 4) && aligned(out_hi, 2) &&
+                    aligned(out_lo, 2),
+                "stb_decode_cross_attn: misaligned q, partial, tickets or output");
+    stb::CrossDecodeKV kv = {(const __half*)k_hi, (const __half*)v_hi};
+    return stb::decode_attn_cross(q, kv, B, H, 64 * H, partial, (int*)tickets, (__half*)out_hi, (__half*)out_lo, out_f32,
+                                  (cudaStream_t)stream);
+}
+
+extern "C" int stb_decode_cross_splits(void) { return stb::decode_cross_splits(); }

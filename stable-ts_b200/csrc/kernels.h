@@ -45,7 +45,6 @@ struct CrossDecodeKV {
 };
 int decode_attn_cross(const float* q, const CrossDecodeKV& kv, int B, int H, int d, float* partial, int* tickets, __half* oh,
                       __half* ol, float* of, cudaStream_t st);
-size_t decode_cross_scratch_bytes(int B, int H);
 int decode_cross_splits();
 int v_headmajor(const __half* vT_hi, int BH, int T, int Tp, __half* v_hi, cudaStream_t st);
 int gemv(const void* x_hi, const void* x_lo, int B, int K, const void* w_hi, const void* w_lo, int N, const float* bias,

@@ -56,7 +56,7 @@ def test_option_switch_and_error_reporting_without_a_gpu():
     with a message (include/stablets_b200.h)."""
     from stable_ts_b200 import _lib as L
     lib = L.lib()
-    assert lib.stb_abi_version() >= 4
+    assert lib.stb_abi_version() >= 5
     assert L.get_option("decode_fused_ln") in (0, 1)
     old = L.get_option("decode_fused_ln")
     L.set_option("decode_fused_ln", 1 - old)
@@ -75,3 +75,8 @@ def test_option_switch_and_error_reporting_without_a_gpu():
     assert lib.stb_axpby(None, None, 1.0, 0.0, 8, None) != 0 and b"stb_axpby" in lib.stb_last_error()
     assert lib.stb_decode_linear(None, None, 48, 100, None, None, 1280, None, 0, None, 0, None, None, None, 1280, None, 0, 0,
                                  None, None, None) != 0 and b"K=100" in lib.stb_last_error()
+    assert lib.stb_decode_self_attn(None, None, None, 4, 0, 448, None, None, None, None, None, None) != 0
+    assert b"stb_decode_self_attn: H=0" in lib.stb_last_error()
+    assert lib.stb_decode_cross_attn(None, None, None, 0, 20, None, None, None, None, None, None) != 0
+    assert b"stb_decode_cross_attn: B=0" in lib.stb_last_error()
+    assert lib.stb_decode_cross_splits() >= 1
