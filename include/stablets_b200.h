@@ -334,6 +334,22 @@ STB_API int stb_decode_cross_attn(const float* q, const void* k_hi, const void* 
                                   float* out_f32, void* out_hi, void* out_lo, void* stream);
 STB_API int stb_decode_cross_splits(void);
 
+/* The LayerNorm and softmax row kernels of the encoder and the teacher-forced decoder on their own, exposed for tests
+ *    (csrc/elementwise.cu).  Split planes are hi = rn(y), lo = rn(y - hi) of the fp32 result y.
+ * stb_layernorm: whisper's LayerNorm of rows x fp32 [rows][d] (row pitch d): statistics in fp32, biased variance, eps 1e-5,
+ *    y = (x - mean) / sqrt(var + 1e-5) gamma + beta.  d a multiple of 128 in 128..1280, rows >= 0.  Outputs (row pitch d):
+ *    out_f32 fp32 and / or the split planes out_hi / out_lo fp16 (out_lo needs out_hi); at least one of out_f32 / out_hi.
+ *    Nothing beyond row `rows` is written.  x, gamma, beta and out_f32 16-byte aligned; out_hi / out_lo 8-byte aligned.
+ * stb_softmax_rows: softmax of attention-score rows S fp32 [n_rows][ld_s] into split planes p_hi / p_lo fp16 [n_rows][ld_p]
+ *    (p_lo may be NULL).  Row r covers its first n_valid(r) columns: min(n_cols, r % rows_per_slice + 1) when causal (the
+ *    decoder's mask over slices of rows_per_slice query rows), n_cols otherwise; columns n_valid(r)..ld_p-1 are written as
+ *    0 and nothing at or beyond ld_p is.  Only columns below n_valid(r) of S are read.  1 <= n_cols <= 1504,
+ *    ld_s >= n_cols, n_cols <= ld_p <= 1504; rows_per_slice >= 1 when causal. */
+STB_API int stb_layernorm(const float* x, long long rows, int d, const float* gamma, const float* beta, void* out_hi, void* out_lo,
+                          float* out_f32, void* stream);
+STB_API int stb_softmax_rows(const float* S, long long n_rows, int n_cols, long long ld_s, int rows_per_slice, int causal,
+                             void* p_hi, void* p_lo, long long ld_p, void* stream);
+
 /* per-sequence sampling state kept on the device */
 typedef struct {
     int32_t n_sampled;   /* tokens sampled so far (0 at sample_begin) */

@@ -93,6 +93,9 @@ _SIGS = {
     "stb_decode_cross_attn": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                       c_void_p, c_void_p]),
     "stb_decode_cross_splits": (c_int, []),
+    "stb_layernorm": (c_int, [c_void_p, c_longlong, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "stb_softmax_rows": (c_int, [c_void_p, c_longlong, c_int, c_longlong, c_int, c_int, c_void_p, c_void_p, c_longlong,
+                                 c_void_p]),
     "stb_sample": (c_int, [c_void_p, c_longlong, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                            c_longlong, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_float, c_void_p,
                            c_void_p, c_void_p]),

@@ -352,3 +352,37 @@ extern "C" int stb_token_probs(const float* logits, long long ld, int n_rows, in
     STB_LAUNCH_OK();
     return STB_OK;
 }
+
+// ---------------------------------------------------------------------------------------------------------
+// test entry points: the LayerNorm and softmax row kernels on their own (include/stablets_b200.h)
+// ---------------------------------------------------------------------------------------------------------
+static bool aligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
+
+extern "C" int stb_layernorm(const float* x, long long rows, int d, const float* gamma, const float* beta, void* out_hi,
+                             void* out_lo, float* out_f32, void* stream) {
+    // one warp per row, d / 128 float4 per lane held in registers (at most 10)
+    STB_REQUIRE(d % 128 == 0 && d >= 128 && d <= 1280, "stb_layernorm: d=%d must be a multiple of 128 in 128..1280", d);
+    STB_REQUIRE(rows >= 0, "stb_layernorm: rows=%lld is negative", rows);
+    STB_REQUIRE(x && gamma && beta, "stb_layernorm: null x, gamma or beta");
+    STB_REQUIRE(out_f32 || out_hi, "stb_layernorm: no output (out_f32 and out_hi are both null)");
+    STB_REQUIRE(out_lo == nullptr || out_hi != nullptr, "stb_layernorm: out_lo needs out_hi");
+    // x, gamma, beta and out_f32 are accessed as float4, the planes as uint2
+    STB_REQUIRE(aligned(x, 16) && aligned(gamma, 16) && aligned(beta, 16) && aligned(out_f32, 16),
+                "stb_layernorm: x, gamma, beta and out_f32 must be 16-byte aligned");
+    STB_REQUIRE(aligned(out_hi, 8) && aligned(out_lo, 8), "stb_layernorm: out_hi and out_lo must be 8-byte aligned");
+    return stb::layernorm(x, rows, d, gamma, beta, (__half*)out_hi, (__half*)out_lo, out_f32, (cudaStream_t)stream);
+}
+
+extern "C" int stb_softmax_rows(const float* S, long long n_rows, int n_cols, long long ld_s, int rows_per_slice, int causal,
+                                void* p_hi, void* p_lo, long long ld_p, void* stream) {
+    // one warp per row, 47 columns per lane held in registers: at most 1504 columns
+    STB_REQUIRE(n_cols >= 1 && n_cols <= stb::SM_MAXV * 32, "stb_softmax_rows: n_cols=%d outside 1..%d", n_cols, stb::SM_MAXV * 32);
+    STB_REQUIRE(ld_s >= n_cols, "stb_softmax_rows: ld_s=%lld < n_cols=%d", ld_s, n_cols);
+    STB_REQUIRE(ld_p >= n_cols && ld_p <= stb::SM_MAXV * 32, "stb_softmax_rows: ld_p=%lld outside n_cols..%d", ld_p,
+                stb::SM_MAXV * 32);
+    STB_REQUIRE(n_rows >= 0, "stb_softmax_rows: n_rows=%lld is negative", n_rows);
+    STB_REQUIRE(!causal || rows_per_slice >= 1, "stb_softmax_rows: rows_per_slice=%d must be positive when causal", rows_per_slice);
+    STB_REQUIRE(S && p_hi, "stb_softmax_rows: null S or p_hi");
+    return stb::softmax_rows(S, n_rows, n_cols, ld_s, rows_per_slice, causal, (__half*)p_hi, (__half*)p_lo, ld_p,
+                             (cudaStream_t)stream);
+}

@@ -129,7 +129,7 @@ extern "C" int stb_axpby(float* y, const float* x, float a, float b, long long n
 }
 
 extern "C" const char* stb_last_error(void) { return stb::get_error(); }
-extern "C" int stb_abi_version(void) { return 5; }
+extern "C" int stb_abi_version(void) { return 6; }
 extern "C" int stb_set_option(const char* name, int value) {
     STB_REQUIRE(name, "stb_set_option: null name");
     stb::opt_init();

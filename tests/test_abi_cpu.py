@@ -56,7 +56,7 @@ def test_option_switch_and_error_reporting_without_a_gpu():
     with a message (include/stablets_b200.h)."""
     from stable_ts_b200 import _lib as L
     lib = L.lib()
-    assert lib.stb_abi_version() >= 5
+    assert lib.stb_abi_version() >= 6
     assert L.get_option("decode_fused_ln") in (0, 1)
     old = L.get_option("decode_fused_ln")
     L.set_option("decode_fused_ln", 1 - old)
@@ -80,3 +80,7 @@ def test_option_switch_and_error_reporting_without_a_gpu():
     assert lib.stb_decode_cross_attn(None, None, None, 0, 20, None, None, None, None, None, None) != 0
     assert b"stb_decode_cross_attn: B=0" in lib.stb_last_error()
     assert lib.stb_decode_cross_splits() >= 1
+    assert lib.stb_layernorm(None, 8, 1408, None, None, None, None, None, None) != 0
+    assert b"stb_layernorm: d=1408" in lib.stb_last_error()
+    assert lib.stb_softmax_rows(None, 8, 1500, 1504, 1, 0, None, None, 1496, None) != 0
+    assert b"stb_softmax_rows: ld_p=1496" in lib.stb_last_error()
