@@ -43,13 +43,6 @@ extern "C" {
 
 STB_API const char* stb_last_error(void);
 STB_API int stb_abi_version(void);
-/* run-time switch for A/B measurement of a kernel variant on the same box (default also from the environment: STB_<NAME>):
- *   "decode_fused_ln"      0/1  LayerNorm folded into the decode-step linears (needs the STB_L_*_WG / *_FOLD tensors;
- *                               STB_PREC_FP16X3 models only, STB_PREC_FP16 models ignore it).
- * stb_set_option rejects an unknown name with an error; stb_get_option returns -1 for it.  Not part of the reference's
- * behaviour -- every setting must pass the same parity tests. */
-STB_API int stb_set_option(const char* name, int value);
-STB_API int stb_get_option(const char* name);
 /* measurement hooks (bench.py): kernels launched by this library so far; per-launch CUDA-event timing of every kernel */
 STB_API unsigned long long stb_launch_count(void);
 STB_API void stb_prof_enable(int on);
@@ -129,19 +122,12 @@ STB_API int stb_gemv(const void* x_hi, const void* x_lo, int B, int K, const voi
  *   out[b][n] = act(sum_k W[n][k] x[b][k] + bias[n]) + res[b][n] for b < B, n < N; nothing else of the outputs is written.
  *   x split planes [B][K] (row pitch K), W split planes [N][K]; lo planes for both or neither (single pass).  B in 1..128,
  *   K a multiple of 64.  Outputs: fp32 and/or split planes (out_lo may be NULL), row pitch ld_out >= N; res may alias
- *   out_f32 (row pitch ld_res >= N).  bias, ln_wsum, res and out_f32 16-byte aligned; out_hi / out_lo 8-byte aligned.
- *   Folded LayerNorm (ln_stats_in != NULL): x is the RAW row and W = W' diag(gamma) (with bias = W' beta + b'):
- *     out = rstd (acc - mean ln_wsum[n]) + bias[n], ln_wsum [N] the row sums of the W planes; the statistics of the
- *     ln_row_features-wide input rows come from ln_stats_in [ln_tiles_in][B][2]: per tile (sum, sum of squares about the
- *     tile's own mean), tile t holding features [128 t, 128 t + 128) (ln_tiles_in = ceil(ln_row_features / 128)) or the
- *     whole row (ln_tiles_in = 1).
- *   stats_out (nullable) [ceil(N / 128)][B][2]: the same per-tile statistics of the final output rows, for the next Linear.
+ *   out_f32 (row pitch ld_res >= N).  bias, res and out_f32 16-byte aligned; out_hi / out_lo 8-byte aligned.
  * stb_decode_linear_split: the cluster size (1..8) stb_decode_linear uses for an N x K weight on the current device, 0 for
  * a bad shape. */
 STB_API int stb_decode_linear(const void* x_hi, const void* x_lo, int B, int K, const void* w_hi, const void* w_lo, int N,
                               const float* bias, int act, const float* res, long long ld_res, float* out_f32, void* out_hi,
-                              void* out_lo, long long ld_out, const float* ln_stats_in, int ln_tiles_in, int ln_row_features,
-                              const float* ln_wsum, float* stats_out, void* stream);
+                              void* out_lo, long long ld_out, void* stream);
 STB_API int stb_decode_linear_split(int n, int k);
 
 /* fp32 [rows][cols] (row pitch src_ld) -> split planes (row pitch dst_ld); lo may be NULL */
@@ -174,23 +160,12 @@ enum {
     STB_T_DEC_POS,         /* f32 [n_text_ctx][d] */
     STB_T_DEC_LN_G,
     STB_T_DEC_LN_B,
-    /* optional, decode step with the final LayerNorm folded into the vocabulary projection (see STB_L_*_WG below) */
-    STB_T_DEC_TOKEMB_G,    /* split [V][d]: token embedding * ln.weight (column-wise) */
-    STB_T_DEC_TOKEMB_FOLD, /* f32 [2][V4], V4 = V rounded up to 4: row sums of the split planes | emb . ln.bias */
     STB_T_LAYER_BASE = 32,
     /* per-layer ids (add to STB_T_LAYER_BASE); encoder layers use ENC_*, decoder layers DEC_* */
     STB_L_ATTN_LN_G = 0, STB_L_ATTN_LN_B, STB_L_QKV_W /* split [3d][d]: q,k,v */, STB_L_QKV_B /* f32 [3d], k part 0 */,
     STB_L_OUT_W, STB_L_OUT_B, STB_L_MLP_LN_G, STB_L_MLP_LN_B, STB_L_FC1_W, STB_L_FC1_B, STB_L_FC2_W, STB_L_FC2_B,
     STB_L_CROSS_LN_G, STB_L_CROSS_LN_B, STB_L_CQ_W, STB_L_CQ_B, STB_L_CKV_W /* split [2d][d]: k,v */,
     STB_L_CKV_B /* f32 [2d], k part 0 */, STB_L_COUT_W, STB_L_COUT_B,
-    /* OPTIONAL (decoder layers): the LayerNorm in front of a decode-step Linear folded into it.  With W' = W diag(g),
-     * y = rstd (W' x - mean * rowsum(W')) + (W beta + bias): the step's GEMM runs on the raw residual stream x, its epilogue
-     * applies the row statistics that the PRODUCER of x left behind -- no LayerNorm launch (3 per layer) in the step.  The
-     * producer leaves, per 128-feature tile of x, the sum and the sum of squares about the TILE mean; the consumer combines
-     * the tiles with Chan's formula (no E[x^2] - mean^2 cancellation for rows far from zero mean).  FP16X3 models only.
-     *   *_WG    split [n][d]   W' (hi / lo planes)
-     *   *_FOLD  f32 [2][n4]    n4 = n rounded up to 4: rowsum of the planes (what the tensor core multiplies) | W beta + bias */
-    STB_L_QKV_WG, STB_L_QKV_FOLD, STB_L_CQ_WG, STB_L_CQ_FOLD, STB_L_FC1_WG, STB_L_FC1_FOLD,
     STB_L_COUNT
 };
 

@@ -16,11 +16,10 @@ N_FRAMES, N_AUDIO_CTX, KPAD = 3000, 1500, 1504
 
 # tensor ids (include/stablets_b200.h)
 (T_ENC_CONV1_W, T_ENC_CONV1_B, T_ENC_CONV2_W, T_ENC_CONV2_B, T_ENC_POS, T_ENC_LNPOST_G, T_ENC_LNPOST_B,
- T_DEC_TOKEMB_F32, T_DEC_TOKEMB, T_DEC_POS, T_DEC_LN_G, T_DEC_LN_B, T_DEC_TOKEMB_G, T_DEC_TOKEMB_FOLD) = range(14)
+ T_DEC_TOKEMB_F32, T_DEC_TOKEMB, T_DEC_POS, T_DEC_LN_G, T_DEC_LN_B) = range(12)
 T_LAYER_BASE = 32
 (L_ATTN_LN_G, L_ATTN_LN_B, L_QKV_W, L_QKV_B, L_OUT_W, L_OUT_B, L_MLP_LN_G, L_MLP_LN_B, L_FC1_W, L_FC1_B, L_FC2_W,
- L_FC2_B, L_CROSS_LN_G, L_CROSS_LN_B, L_CQ_W, L_CQ_B, L_CKV_W, L_CKV_B, L_COUT_W, L_COUT_B, L_QKV_WG, L_QKV_FOLD, L_CQ_WG,
- L_CQ_FOLD, L_FC1_WG, L_FC1_FOLD, L_COUNT) = range(27)
+ L_FC2_B, L_CROSS_LN_G, L_CROSS_LN_B, L_CQ_W, L_CQ_B, L_CKV_W, L_CKV_B, L_COUT_W, L_COUT_B, L_COUNT) = range(21)
 
 
 class Operand(ctypes.Structure):
@@ -43,8 +42,6 @@ class Dims(ctypes.Structure):
 _SIGS = {
     "stb_last_error": (c_char_p, []),
     "stb_abi_version": (c_int, []),
-    "stb_set_option": (c_int, [c_char_p, c_int]),
-    "stb_get_option": (c_int, [c_char_p]),
     "stb_launch_count": (ctypes.c_ulonglong, []),
     "stb_prof_enable": (None, [c_int]),
     "stb_prof_report": (c_int, [ctypes.c_char_p, c_size_t]),
@@ -60,8 +57,7 @@ _SIGS = {
     "stb_gemv": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_longlong,
                          c_void_p, c_void_p, c_void_p, c_longlong, c_void_p]),
     "stb_decode_linear": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p,
-                                  c_longlong, c_void_p, c_void_p, c_void_p, c_longlong, c_void_p, c_int, c_int, c_void_p,
-                                  c_void_p, c_void_p]),
+                                  c_longlong, c_void_p, c_void_p, c_void_p, c_longlong, c_void_p]),
     "stb_decode_linear_split": (c_int, [c_int, c_int]),
     "stb_split_f16": (c_int, [c_void_p, c_longlong, c_int, c_longlong, c_void_p, c_void_p, c_longlong, c_void_p]),
     "stb_model_create": (c_int, [POINTER(Dims), c_int, POINTER(c_void_p)]),
@@ -144,14 +140,9 @@ def check(rc: int):
         raise StbError(f"libstablets_b200 error {rc}: {lib().stb_last_error().decode(errors='replace')}")
 
 
-def set_option(name: str, value: int):
-    """Run-time kernel-variant switch (stb_set_option): "decode_fused_ln" (LayerNorm folded into the decode-step linears).
-    An unknown name raises StbError."""
-    check(lib().stb_set_option(name.encode(), int(value)))
-
-
 def get_option(name: str) -> int:
-    return int(lib().stb_get_option(name.encode()))
+    """-1 for every name: the library has no kernel-variant switches; kept for callers that report option values."""
+    return -1
 
 
 def ptr(t):

@@ -83,10 +83,6 @@ __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;"
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
 bool pdl_enabled(int kind = 0);   // STB_PDL bit mask (misc.cu): kind 0 = ordinary kernels, 1 = decode_linear
-// run-time switches (stb_set_option / stb_get_option, misc.cu); defaults come from the environment variable of the same
-// meaning so a whole process can be flipped without code (STB_DECODE_FUSED_LN)
-enum Option { OPT_DECODE_FUSED_LN = 0, OPT_COUNT };
-int option(Option o);
 // launch priority of the kernels launched next by this host thread (cudaLaunchAttributePriority; 0 = the stream's own).
 // The decode step raises it for its latency-bound linear layers: under programmatic dependent launch the next kernel's CTAs
 // can become resident while the previous kernel's tail still runs, and the block scheduler then serves the higher-priority
@@ -122,11 +118,6 @@ static inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 b
 // warp helpers
 // ---------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-__device__ __forceinline__ double warp_sum_d(double v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     return v;

@@ -362,8 +362,7 @@ __global__ void __launch_bounds__(256) v_headmajor_kernel(const __half* __restri
 
 __global__ void embed_step_kernel(const int32_t* __restrict__ tokens, const int32_t* __restrict__ pos_ptr,
                                   const int32_t* __restrict__ seq_off, int n_pos, int d, const float* __restrict__ emb,
-                                  const float* __restrict__ posemb, float* __restrict__ x, __half* __restrict__ xs_hi,
-                                  __half* __restrict__ xs_lo, float* __restrict__ stats) {
+                                  const float* __restrict__ posemb, float* __restrict__ x) {
     const int b = blockIdx.x;
     pdl_trigger();
     pdl_wait();
@@ -373,39 +372,9 @@ __global__ void embed_step_kernel(const int32_t* __restrict__ tokens, const int3
     const float4* e = reinterpret_cast<const float4*>(emb + (long long)tokens[b] * d);
     const float4* p = reinterpret_cast<const float4*>(posemb + (long long)pos * d);
     float4* o = reinterpret_cast<float4*>(x + (long long)b * d);
-    float s1 = 0.f;
     for (int i = threadIdx.x; i < (d >> 2); i += blockDim.x) {
         const float4 a = __ldg(e + i), c = __ldg(p + i);
-        const float4 v = make_float4(a.x + c.x, a.y + c.y, a.z + c.z, a.w + c.w);
-        o[i] = v;
-        if (xs_hi != nullptr) {                              // raw-row planes + statistics for the folded LayerNorm of layer 0
-            __half h[4], l[4];
-            split_f16(v.x, h[0], l[0]); split_f16(v.y, h[1], l[1]); split_f16(v.z, h[2], l[2]); split_f16(v.w, h[3], l[3]);
-            reinterpret_cast<uint2*>(xs_hi + (long long)b * d)[i] = *reinterpret_cast<const uint2*>(h);
-            if (xs_lo != nullptr) reinterpret_cast<uint2*>(xs_lo + (long long)b * d)[i] = *reinterpret_cast<const uint2*>(l);
-        }
-        s1 += (v.x + v.y) + (v.z + v.w);
-    }
-    if (stats != nullptr) {                                  // (sum, sum of squares about the row mean): two passes
-        __shared__ float r1[4], r2[4];
-        s1 = warp_sum(s1);
-        if ((threadIdx.x & 31) == 0) r1[threadIdx.x >> 5] = s1;
-        __syncthreads();
-        const float sum = (r1[0] + r1[1]) + (r1[2] + r1[3]);
-        const float mean = sum / (float)d;
-        float q = 0.f;
-        for (int i = threadIdx.x; i < (d >> 2); i += blockDim.x) {
-            const float4 v = o[i];                           // this thread's own stores above
-            const float a = v.x - mean, bb = v.y - mean, c = v.z - mean, w = v.w - mean;
-            q += (a * a + bb * bb) + (c * c + w * w);
-        }
-        q = warp_sum(q);
-        if ((threadIdx.x & 31) == 0) r2[threadIdx.x >> 5] = q;
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            stats[2 * b] = sum;
-            stats[2 * b + 1] = (r2[0] + r2[1]) + (r2[2] + r2[3]);
-        }
+        o[i] = make_float4(a.x + c.x, a.y + c.y, a.z + c.z, a.w + c.w);
     }
 }
 
@@ -666,9 +635,8 @@ int v_headmajor(const __half* vT_hi, int BH, int T, int Tp, __half* v_hi, cudaSt
     return STB_OK;
 }
 int embed_step(const int32_t* tokens, const int32_t* pos, const int32_t* seq_off, int n_pos, int B, int d, const float* emb,
-               const float* posemb, float* x, __half* xs_hi, __half* xs_lo, float* stats, cudaStream_t st) {
-    STB_CUDA_OK(launch_pdl(embed_step_kernel, dim3(B), dim3(128), 0, st, tokens, pos, seq_off, n_pos, d, emb, posemb, x, xs_hi, xs_lo,
-                           stats));
+               const float* posemb, float* x, cudaStream_t st) {
+    STB_CUDA_OK(launch_pdl(embed_step_kernel, dim3(B), dim3(128), 0, st, tokens, pos, seq_off, n_pos, d, emb, posemb, x));
     STB_LAUNCH_OK();
     return STB_OK;
 }

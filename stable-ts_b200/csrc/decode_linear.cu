@@ -34,16 +34,6 @@ struct DLArgs {
     __half* out_hi;
     __half* out_lo;
     long long ld_out;
-    // LayerNorm folded into this Linear (DLFuse): out = rstd_s (acc - mean_s wsum[n]) + bias[n], the row statistics of
-    // sequence s combined from ln_tiles partial (sum, sum of squares about the tile mean) pairs [ln_tiles][B][2] left by
-    // the producer of x: 128-feature tiles, or the whole row when ln_tiles == 1
-    const float* ln_stats;
-    int ln_tiles;
-    int ln_features;          // features of the normalised row
-    const float* ln_wsum;     // [n]
-    // this Linear produces a row that the NEXT Linear normalises: per 128-feature tile the (sum, sum of squares about the
-    // tile mean) of the final values (after bias / activation / residual) of every sequence, [tiles][B][2]
-    float* stats_out;
 };
 
 __device__ __forceinline__ uint32_t cluster_rank() {
@@ -221,8 +211,8 @@ decode_linear_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_cons
         // Reduce-scatter over distributed shared memory: rank r owns sequences [r BN / split, (r + 1) BN / split).  A warp
         // handles one sequence per iteration, a lane 4 consecutive features of it: it issues the 16-byte loads of ALL peers
         // first (independent, so their DSMEM latencies overlap), adds them in rank order (bit-reproducible), applies the
-        // epilogue and stores 16 bytes.  Every lane walks the loop (warp-uniform bounds): the folded LayerNorm and the row
-        // statistics below are warp reductions.
+        // epilogue and stores 16 bytes.  The loop bounds are warp-uniform; lanes whose features lie past n skip their
+        // global loads and stores.
         const int e = warp * 32 + lane;                        // 0 .. 255
         const int quad = e & 31;                               // features m0 + 4 quad .. + 3
         const int m = m0 + quad * 4;
@@ -231,7 +221,7 @@ decode_linear_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_cons
         uint32_t peer[8];
 #pragma unroll
         for (int p = 0; p < 8; ++p) peer[p] = p < split ? dsmem_addr(local, (uint32_t)p) : 0u;
-        pdl_wait();                                             // residual and row statistics are earlier kernels' outputs
+        pdl_wait();                                             // the residual is an earlier kernel's output
         const bool full = m + 3 < g.n;                          // all 4 features exist
         const bool vec = full && (g.ld_out & 3) == 0 && (g.res == nullptr || (g.ld_res & 3) == 0);
         auto load4 = [&](const float* p) -> float4 {            // 4 per-feature constants, zero past n
@@ -244,8 +234,6 @@ decode_linear_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_cons
             return r;
         };
         const float4 bias = load4(g.bias);
-        const float4 wsum = load4(g.ln_wsum);
-        const int tile = blockIdx.x / split;
         for (int c = c0 + (e >> 5); c < c1 && c < g.B; c += 8) {
             const uint32_t off = (uint32_t)((c * 128 + quad * 4) * 4);
             float4 v[8];
@@ -256,27 +244,6 @@ decode_linear_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_cons
 #pragma unroll
             for (int p = 1; p < 8; ++p)
                 if (p < split) { a.x += v[p].x; a.y += v[p].y; a.z += v[p].z; a.w += v[p].w; }
-            if (g.ln_stats != nullptr) {                        // folded LayerNorm of the input row of sequence c
-                // Chan et al.'s combination of the tiles' (sum s_t, squared deviations M2_t) over their n_t features:
-                //   M2 = sum_t M2_t + n_t (s_t / n_t - mean)^2 -- no E[x^2] - mean^2 cancellation for rows far from zero
-                //   mean.  Lane t holds tile t; the shuffle trees are fixed and commutative: every lane gets the same bits.
-                double s = 0.0, m2 = 0.0;
-                int nt = 0;
-                if (quad < g.ln_tiles) {
-                    const float2 pr = *reinterpret_cast<const float2*>(g.ln_stats + ((long long)quad * g.B + c) * 2);
-                    s = pr.x;
-                    m2 = pr.y;
-                    nt = g.ln_tiles == 1 ? g.ln_features : min(128, g.ln_features - 128 * quad);
-                }
-                const double inv_n = 1.0 / (double)g.ln_features;
-                const double mu = warp_sum_d(s) * inv_n;
-                const double dev = nt > 0 ? s / (double)nt - mu : 0.0;
-                const double var = warp_sum_d(m2 + (double)nt * dev * dev) * inv_n;
-                const float rstd = (float)(1.0 / sqrt(var + 1e-5));
-                const float muf = (float)mu;
-                a.x = (a.x - muf * wsum.x) * rstd; a.y = (a.y - muf * wsum.y) * rstd;
-                a.z = (a.z - muf * wsum.z) * rstd; a.w = (a.w - muf * wsum.w) * rstd;
-            }
             a.x += bias.x; a.y += bias.y; a.z += bias.z; a.w += bias.w;
             if (g.act == STB_ACT_GELU) { a.x = gelu_erf(a.x); a.y = gelu_erf(a.y); a.z = gelu_erf(a.z); a.w = gelu_erf(a.w); }
             if (g.res != nullptr) {
@@ -290,22 +257,6 @@ decode_linear_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_cons
                     if (m + 2 < g.n) a.z += rp[2];
                     if (m + 3 < g.n) a.w += rp[3];
                 }
-            }
-            if (g.stats_out != nullptr) {                       // partial row statistics of this 128-feature tile
-                float s1 = 0.f;
-                if (m < g.n) s1 += a.x;
-                if (m + 1 < g.n) s1 += a.y;
-                if (m + 2 < g.n) s1 += a.z;
-                if (m + 3 < g.n) s1 += a.w;
-                s1 = warp_sum(s1);
-                const float mt = s1 / (float)min(128, g.n - m0);   // tile mean: the squares are taken about it (two pass)
-                float q = 0.f, t;
-                if (m < g.n) { t = a.x - mt; q += t * t; }
-                if (m + 1 < g.n) { t = a.y - mt; q += t * t; }
-                if (m + 2 < g.n) { t = a.z - mt; q += t * t; }
-                if (m + 3 < g.n) { t = a.w - mt; q += t * t; }
-                q = warp_sum(q);
-                if (quad == 0) *reinterpret_cast<float2*>(g.stats_out + ((long long)tile * g.B + c) * 2) = make_float2(s1, q);
             }
             const long long off_o = (long long)c * g.ld_out + m;
             if (vec) {
@@ -399,7 +350,7 @@ static int launch_dl(const TmapVal& wh, const TmapVal& wl, const TmapVal& xh, co
 // out[B][n] = epilogue(x[B][k] . W[n][k]^T); x / W split-fp16 planes, K-major; B <= 128; k a multiple of 64.
 int decode_linear(const void* x_hi, const void* x_lo, int B, int k, const void* w_hi, const void* w_lo, int n, const float* bias,
                   int act, const float* res, long long ld_res, float* out_f32, void* out_hi, void* out_lo, long long ld_out,
-                  const DLFuse* fuse, cudaStream_t st) {
+                  cudaStream_t st) {
     STB_REQUIRE(x_hi && w_hi && (out_f32 || out_hi), "decode_linear: null argument");
     STB_REQUIRE(B >= 1 && B <= 128 && k % 64 == 0 && n >= 1, "decode_linear: unsupported shape B=%d k=%d n=%d", B, k, n);
     STB_REQUIRE((x_lo != nullptr) == (w_lo != nullptr), "decode_linear: lo planes must be given for both operands or neither");
@@ -409,16 +360,6 @@ int decode_linear(const void* x_hi, const void* x_lo, int B, int k, const void* 
     g.n = n; g.B = B; g.kb_total = k / 64;
     g.bias = bias; g.act = act; g.res = res; g.ld_res = ld_res;
     g.out_f32 = out_f32; g.out_hi = (__half*)out_hi; g.out_lo = (__half*)out_lo; g.ld_out = ld_out;
-    if (fuse != nullptr) {
-        if (fuse->stats_in != nullptr) {
-            STB_REQUIRE(fuse->wsum != nullptr && fuse->tiles_in >= 1 && fuse->tiles_in <= 32 && fuse->row_features >= 1 &&
-                            (fuse->tiles_in == 1 || fuse->tiles_in == cdiv(fuse->row_features, 128)),
-                        "decode_linear: folded LayerNorm needs wsum and 1 or ceil(features / 128) <= 32 statistic tiles");
-            g.ln_stats = fuse->stats_in; g.ln_tiles = fuse->tiles_in; g.ln_features = fuse->row_features;
-            g.ln_wsum = fuse->wsum;
-        }
-        g.stats_out = fuse->stats_out;
-    }
     const int split = decode_linear_split(n, k);
     TmapVal wh, wl, xh, xl;
     STB_TRY(make_tmap(w_hi, n, k, 1, 1, k, 0, 0, 128, &wh));
@@ -448,8 +389,7 @@ static bool aligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<u
 
 extern "C" int stb_decode_linear(const void* x_hi, const void* x_lo, int B, int K, const void* w_hi, const void* w_lo, int N,
                                  const float* bias, int act, const float* res, long long ld_res, float* out_f32, void* out_hi,
-                                 void* out_lo, long long ld_out, const float* ln_stats_in, int ln_tiles_in, int ln_row_features,
-                                 const float* ln_wsum, float* stats_out, void* stream) {
+                                 void* out_lo, long long ld_out, void* stream) {
     STB_REQUIRE(B >= 1 && B <= 128, "stb_decode_linear: B=%d outside 1..128", B);
     STB_REQUIRE(K >= 64 && K % 64 == 0, "stb_decode_linear: K=%d must be a positive multiple of 64", K);
     STB_REQUIRE(N >= 1, "stb_decode_linear: N=%d must be positive", N);
@@ -457,18 +397,11 @@ extern "C" int stb_decode_linear(const void* x_hi, const void* x_lo, int B, int 
     STB_REQUIRE(act == STB_ACT_NONE || act == STB_ACT_GELU, "stb_decode_linear: unknown activation %d", act);
     STB_REQUIRE(x_hi && w_hi && (out_f32 || out_hi) && (out_lo == nullptr || out_hi != nullptr), "stb_decode_linear: null argument");
     STB_REQUIRE((x_lo != nullptr) == (w_lo != nullptr), "stb_decode_linear: lo planes must be given for both operands or neither");
-    STB_REQUIRE(ln_stats_in == nullptr ||
-                    (ln_wsum != nullptr && ln_tiles_in >= 1 && ln_tiles_in <= 32 && ln_row_features >= 1 &&
-                     (ln_tiles_in == 1 || ln_tiles_in == stb::cdiv(ln_row_features, 128))),
-                "stb_decode_linear: a folded LayerNorm needs ln_wsum and 1 (whole row) or ceil(%d / 128) statistic tiles, got %d",
-                ln_row_features, ln_tiles_in);
-    // vector loads / stores: per-feature constants and fp32 rows as float4, fp16 rows as 4 halves, statistics as float2
-    STB_REQUIRE(aligned(bias, 16) && aligned(ln_wsum, 16) && aligned(res, 16) && aligned(out_f32, 16) && aligned(out_hi, 8) &&
-                    aligned(out_lo, 8) && aligned(ln_stats_in, 8) && aligned(stats_out, 8),
+    // vector loads / stores: per-feature constants and fp32 rows as float4, fp16 rows as 4 halves
+    STB_REQUIRE(aligned(bias, 16) && aligned(res, 16) && aligned(out_f32, 16) && aligned(out_hi, 8) && aligned(out_lo, 8),
                 "stb_decode_linear: misaligned pointer");
-    stb::DLFuse fuse = {ln_stats_in, ln_stats_in ? ln_tiles_in : 0, ln_stats_in ? ln_row_features : 0, ln_wsum, stats_out};
     return stb::decode_linear(x_hi, x_lo, B, K, w_hi, w_lo, N, bias, act, res, ld_res, out_f32, out_hi, out_lo, ld_out,
-                              (ln_stats_in || stats_out) ? &fuse : nullptr, (cudaStream_t)stream);
+                              (cudaStream_t)stream);
 }
 
 extern "C" int stb_decode_linear_split(int n, int k) {

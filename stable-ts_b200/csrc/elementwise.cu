@@ -1,5 +1,5 @@
 // K5 / K9: bandwidth-bound row kernels around the GEMMs -- LayerNorm, softmax (plain / causal), token embedding,
-// mel repack for conv-as-GEMM, im2col, cross-attention capture copy, token probability + rank.
+// mel repack for conv-as-GEMM, cross-attention capture copy, token probability + rank.
 // All use one warp per row with 128-bit global accesses and warp-shuffle reductions; outputs that feed a GEMM are
 // written directly as split-fp16 planes so no separate conversion pass touches HBM.
 #include "common.cuh"
@@ -208,29 +208,6 @@ __global__ void zero_pad_rows_kernel(__half* hi, __half* lo, int C, int T) {
 }
 int zero_pad_rows(__half* hi, __half* lo, int B, int C, int T, cudaStream_t st) {
     zero_pad_rows_kernel<<<B, 256, 0, st>>>(hi, lo, C, T);
-    STB_LAUNCH_OK();
-    return STB_OK;
-}
-
-// explicit im2col (used only when the overlapping-row TMA view is disabled): dst[b][t][tap*C + c] = src[b][t*stride+tap][c]
-__global__ void im2col3_kernel(const __half* __restrict__ src, int C, int Tin_pad, int Tout, int stride,
-                               __half* __restrict__ dst) {
-    const int b = blockIdx.y;
-    const long long n8 = (long long)Tout * 3 * C / 8;
-    const uint4* s = reinterpret_cast<const uint4*>(src + (long long)b * Tin_pad * C);
-    uint4* d = reinterpret_cast<uint4*>(dst + (long long)b * Tout * 3 * C);
-    const int row8 = 3 * C / 8, c8 = C / 8;
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n8; i += (long long)gridDim.x * blockDim.x) {
-        const int t = (int)(i / row8);
-        const int k = (int)(i - (long long)t * row8);
-        const int tap = k / c8, c = k - tap * c8;
-        d[i] = s[(long long)(t * stride + tap) * c8 + c];
-    }
-}
-int im2col3(const __half* src, int B, int C, int Tin_pad, int Tout, int stride, __half* dst, cudaStream_t st) {
-    STB_REQUIRE(C % 8 == 0, "im2col3: C %% 8 != 0");
-    dim3 grid(min(cdiv((long long)Tout * 3 * C / 8, 256), 2048), B);
-    im2col3_kernel<<<grid, 256, 0, st>>>(src, C, Tin_pad, Tout, stride, dst);
     STB_LAUNCH_OK();
     return STB_OK;
 }

@@ -12,7 +12,6 @@
 //   V                        stored transposed [B][H][64][ldk] so P.V is a K-major GEMM
 //   conv inputs              time-major [B][T+2][C] with zero pad rows: overlapping TMA rows (stride C or 2C, width 3C)
 //                            are the im2col matrix, no copy
-#include <stdlib.h>
 #include <string.h>
 #include <vector>
 
@@ -22,7 +21,6 @@
 struct stb_model {
     stb_dims dims;
     int prec;
-    bool conv_im2col;
     const void* t[STB_T_LAYER_BASE][2];
     struct Layer { const void* p[STB_L_COUNT][2]; };
     std::vector<Layer> enc, dec;
@@ -128,27 +126,22 @@ static int linear(const stb_model* m, const Split& x, long long rows, int k, con
 // encoder
 // ---------------------------------------------------------------------------------------------------------
 struct EncWs {
-    Split melT, h1, col, ln, qk, vT, P, attn, hid;
+    Split melT, h1, ln, qk, vT, attn, hid;
     float* x;
-    float* S;
     size_t bytes;
 };
 static EncWs carve_encoder(const stb_model* m, int B, void* ws) {
     const stb_dims& D = m->dims;
     const bool lo = m->prec == STB_PREC_FP16X3;
-    const size_t T = D.n_audio_ctx, Tp = STB_KPAD, d = D.n_audio_state, H = D.n_audio_head, C = D.n_mels;
+    const size_t T = D.n_audio_ctx, Tp = STB_KPAD, d = D.n_audio_state, C = D.n_mels;
     Carver c(ws);
     EncWs w;
     w.melT = take_split(c, (size_t)B * (STB_N_FRAMES + 2) * C, lo);
     w.h1 = take_split(c, (size_t)B * (STB_N_FRAMES + 2) * d, lo);
-    w.col = m->conv_im2col ? take_split(c, (size_t)B * STB_N_FRAMES * 3 * (C > d / 2 ? C : d / 2) + 64, lo) : Split{nullptr, nullptr};
     w.x = c.take<float>((size_t)B * T * d);
     w.ln = take_split(c, (size_t)B * T * d, lo);
     w.qk = take_split(c, (size_t)B * T * 2 * d, lo);
     w.vT = take_split(c, (size_t)B * d * Tp, lo);
-    const bool unfused = getenv("STB_UNFUSED_ATTENTION") != nullptr;   // debugging aid: scores/probabilities through HBM
-    w.S = unfused ? c.take<float>((size_t)B * H * T * Tp) : nullptr;
-    w.P = unfused ? take_split(c, (size_t)B * H * T * Tp, lo) : Split{nullptr, nullptr};
     w.attn = take_split(c, (size_t)B * T * d, lo);
     w.hid = take_split(c, (size_t)B * T * 4 * d, lo);
     w.bytes = c.off;
@@ -170,15 +163,8 @@ static int encoder_forward(stb_model* m, const float* mel, int B, float* xa_f32,
         Split out = {offs(w.h1.hi, d), offs(w.h1.lo, d)};                       // skip the leading pad row
         stb_epilogue e = ep_split(out, d, (const float*)t[STB_T_ENC_CONV1_B][0], STB_ACT_GELU, 0, (long long)(F + 2) * d);
         stb_operand wt = opnd(t[STB_T_ENC_CONV1_W][0], lo ? t[STB_T_ENC_CONV1_W][1] : nullptr, d, 3 * C, 3 * C);
-        if (!m->conv_im2col) {
-            stb_operand a = opnd(w.melT.hi, w.melT.lo, F, 3 * C, C, 0, (long long)(F + 2) * C);
-            STB_TRY(gemm(a, wt, B, 1, e, st));
-        } else {
-            STB_TRY(im2col3(w.melT.hi, B, C, F + 2, F, 1, w.col.hi, st));
-            if (lo) STB_TRY(im2col3(w.melT.lo, B, C, F + 2, F, 1, w.col.lo, st));
-            stb_operand a = opnd(w.col.hi, w.col.lo, F, 3 * C, 3 * C, 0, (long long)F * 3 * C);
-            STB_TRY(gemm(a, wt, B, 1, e, st));
-        }
+        stb_operand a = opnd(w.melT.hi, w.melT.lo, F, 3 * C, C, 0, (long long)(F + 2) * C);
+        STB_TRY(gemm(a, wt, B, 1, e, st));
     }
     // conv2 (k=3, stride 2, pad 1) + GELU + sinusoidal positions -> residual stream x [B][1500][d]
     {
@@ -187,15 +173,8 @@ static int encoder_forward(stb_model* m, const float* mel, int B, float* xa_f32,
         e.out_b_stride = (long long)T * d;
         e.res_b_stride = 0;
         stb_operand wt = opnd(t[STB_T_ENC_CONV2_W][0], lo ? t[STB_T_ENC_CONV2_W][1] : nullptr, d, 3 * d, 3 * d);
-        if (!m->conv_im2col) {
-            stb_operand a = opnd(w.h1.hi, w.h1.lo, T, 3 * d, 2 * d, 0, (long long)(F + 2) * d);
-            STB_TRY(gemm(a, wt, B, 1, e, st));
-        } else {
-            STB_TRY(im2col3(w.h1.hi, B, d, F + 2, T, 2, w.col.hi, st));
-            if (lo) STB_TRY(im2col3(w.h1.lo, B, d, F + 2, T, 2, w.col.lo, st));
-            stb_operand a = opnd(w.col.hi, w.col.lo, T, 3 * d, 3 * d, 0, (long long)T * 3 * d);
-            STB_TRY(gemm(a, wt, B, 1, e, st));
-        }
+        stb_operand a = opnd(w.h1.hi, w.h1.lo, T, 3 * d, 2 * d, 0, (long long)(F + 2) * d);
+        STB_TRY(gemm(a, wt, B, 1, e, st));
     }
     const long long rows = (long long)B * T;
     for (int l = 0; l < D.n_audio_layer; ++l) {
@@ -208,13 +187,9 @@ static int encoder_forward(stb_model* m, const float* mel, int B, float* xa_f32,
                            W_F32(L, STB_L_QKV_B) + 2 * d, w.vT, Tp, st));
         stb_operand q = opnd(w.qk.hi, w.qk.lo, T, 64, 2 * d, 64, (long long)T * 2 * d);
         stb_operand k = opnd(offs(w.qk.hi, d), offs(w.qk.lo, d), T, 64, 2 * d, 64, (long long)T * 2 * d);
-        if (w.S != nullptr) {
-            AttnBufs ab = {w.S, w.P, w.vT, w.attn};
-            STB_TRY(attention(m, B, H, d, T, T, Tp, q, k, ab, 0, st));
-        } else {                                                   // fused wgmma attention: scores never leave the SM
-            stb_operand v = opnd(w.vT.hi, w.vT.lo, 64, Tp, Tp, 64LL * Tp, (long long)d * Tp);
-            STB_TRY(fused_attention(q, k, v, B, H, T, T, w.attn.hi, w.attn.lo, d, 64, (long long)T * d, st));
-        }
+        stb_operand v = opnd(w.vT.hi, w.vT.lo, 64, Tp, Tp, 64LL * Tp, (long long)d * Tp);
+        // fused wgmma attention: scores never leave the SM
+        STB_TRY(fused_attention(q, k, v, B, H, T, T, w.attn.hi, w.attn.lo, d, 64, (long long)T * d, st));
         STB_TRY(linear(m, w.attn, rows, d, W_HI(L, STB_L_OUT_W), W_LO(L, STB_L_OUT_W), d,
                        ep_f32(w.x, d, W_F32(L, STB_L_OUT_B), w.x, d), st));
         STB_TRY(layernorm(w.x, rows, d, W_F32(L, STB_L_MLP_LN_G), W_F32(L, STB_L_MLP_LN_B), w.ln.hi, w.ln.lo, nullptr, st));
@@ -403,8 +378,6 @@ struct StepWs {
     float* xpart;      // cross-attention split partials + tickets
     int* tickets;
     Split ln, attn, hid;
-    Split xs;          // split planes of the raw residual stream x (LayerNorm folded into the consumer, OPT_DECODE_FUSED_LN)
-    float* stats;      // [16][B][2]: per 128-feature tile (sum, sum of squares about the tile mean) of every row of x
     size_t bytes;
 };
 constexpr int STEP_GEMV_MAX_B = 16;      // <= : mma.sync batched GEMV; above: the cluster split-K wgmma kernel
@@ -422,8 +395,6 @@ static StepWs carve_step(const stb_model* m, int B, void* ws) {
     w.ln = take_split(c, (size_t)B * d, lo);
     w.attn = take_split(c, (size_t)B * d, lo);
     w.hid = take_split(c, (size_t)B * 4 * d, lo);
-    w.xs = take_split(c, (size_t)B * d, lo);
-    w.stats = c.take<float>((size_t)16 * B * 2);
     w.bytes = c.off;
     return w;
 }
@@ -460,31 +431,16 @@ static int decode_step(stb_model* m, const int32_t* tokens, int B, int32_t* pos,
         explicit PriorityScope(int p) : saved(launch_priority()) { launch_priority() = p; }
         ~PriorityScope() { launch_priority() = saved; }
     };
-    // LayerNorm folded into the consumer linears (decode_linear.cu, DLFuse): only on the cluster-kernel route, only when the
-    // folded weights were supplied for every layer and the width is a whole number of 128-feature tiles.  Only in FP16X3:
-    // with one fp16 plane the folded GEMM multiplies the raw, un-centred row, whose rounding error after centring grows
-    // as 2^-11 |mean| / std, where the LayerNorm kernels round the normalised row (2^-11)
-    bool fused_ln = option(OPT_DECODE_FUSED_LN) != 0 && m->prec == STB_PREC_FP16X3 && use_splitk && d % 128 == 0 && d / 128 <= 16 &&
-                    t[STB_T_DEC_TOKEMB_G][0] != nullptr && t[STB_T_DEC_TOKEMB_FOLD][0] != nullptr;
-    for (int l = 0; fused_ln && l < D.n_text_layer; ++l)
-        for (int id = STB_L_QKV_WG; id < STB_L_COUNT; ++id)
-            if (m->dec[l].p[id][0] == nullptr) fused_ln = false;
     STB_TRY(embed_step(tokens, pos, seq_off, D.n_text_ctx, B, d, (const float*)t[STB_T_DEC_TOKEMB_F32][0],
-                       (const float*)t[STB_T_DEC_POS][0], w.x, fused_ln ? w.xs.hi : nullptr, fused_ln ? w.xs.lo : nullptr,
-                       fused_ln ? w.stats : nullptr, st));
+                       (const float*)t[STB_T_DEC_POS][0], w.x, st));
     auto lin = [&](const Split& x, int k, const void* w_hi, const void* w_lo, int n, const float* bias, int act,
                    const float* res, float* out_f32, Split out_split, long long ld, const float* ln_g,
-                   const float* ln_b, const DLFuse* fuse = nullptr) -> int {
+                   const float* ln_b) -> int {
         PriorityScope prio(lin_priority);
-        const bool cluster = use_splitk && k % 64 == 0 && n >= 128;
-        if (fuse != nullptr) {                                 // folded LayerNorm: always the cluster kernel
-            STB_REQUIRE(cluster, "decode_step: folded LayerNorm off the cluster route");
-            return decode_linear(x.hi, x.lo, B, k, w_hi, w_lo, n, bias, act, res, ld, out_f32, out_split.hi, out_split.lo, ld, fuse, st);
-        }
         if (use_gemv) {
             STB_TRY(gemv(x.hi, x.lo, B, k, w_hi, w_lo, n, bias, act, res, ld, out_f32, out_split.hi, out_split.lo, ld, st));
-        } else if (cluster) {
-            STB_TRY(decode_linear(x.hi, x.lo, B, k, w_hi, w_lo, n, bias, act, res, ld, out_f32, out_split.hi, out_split.lo, ld, nullptr, st));
+        } else if (use_splitk && k % 64 == 0 && n >= 128) {
+            STB_TRY(decode_linear(x.hi, x.lo, B, k, w_hi, w_lo, n, bias, act, res, ld, out_f32, out_split.hi, out_split.lo, ld, st));
         } else {
             stb_epilogue e;
             memset(&e, 0, sizeof(e));
@@ -498,53 +454,6 @@ static int decode_step(stb_model* m, const int32_t* tokens, int B, int32_t* pos,
     };
     const float* final_g = (const float*)t[STB_T_DEC_LN_G][0];
     const float* final_b = (const float*)t[STB_T_DEC_LN_B][0];
-    if (fused_ln) {
-        // x (fp32) + its split planes + per-tile row statistics travel from producer to consumer; every LayerNorm is the
-        // consumer's epilogue: 8 launches per layer instead of 11
-        const int tiles_d = d / 128;
-        const bool x3 = m->prec == STB_PREC_FP16X3;
-        int tiles_in = 1;                                      // embed_step left full-row sums
-        auto fold = [&](const stb_model::Layer& L, int wg, int fd, int n, DLFuse& f, const void*& whi, const void*& wlo,
-                        const float*& cb) {
-            whi = L.p[wg][0];
-            wlo = x3 ? L.p[wg][1] : nullptr;
-            const float* fp = (const float*)L.p[fd][0];
-            f.stats_in = w.stats; f.tiles_in = tiles_in; f.row_features = d; f.wsum = fp; f.stats_out = nullptr;
-            cb = fp + ((n + 3) & ~3);                          // *_FOLD is f32 [2][n rounded up to 4]
-        };
-        for (int l = 0; l < D.n_text_layer; ++l) {
-            const stb_model::Layer& L = m->dec[l];
-            float* Kc = (float*)state + (size_t)l * 2 * cache;
-            float* Vc = Kc + cache;
-            DLFuse f, prod = {nullptr, 0, 0, nullptr, w.stats};
-            const void *whi, *wlo;
-            const float* cb;
-            fold(L, STB_L_QKV_WG, STB_L_QKV_FOLD, 3 * d, f, whi, wlo, cb);
-            STB_TRY(lin(w.xs, d, whi, wlo, 3 * d, cb, STB_ACT_NONE, nullptr, w.qkv, none, 3 * d, nullptr, nullptr, &f));
-            STB_TRY(decode_attn_self(w.qkv, Kc, Vc, B, H, d, ctx, pos, seq_off, w.attn.hi, w.attn.lo, nullptr, st));
-            STB_TRY(lin(w.attn, d, W_HI(L, STB_L_OUT_W), W_LO(L, STB_L_OUT_W), d, W_F32(L, STB_L_OUT_B), STB_ACT_NONE, w.x, w.x,
-                        w.xs, d, nullptr, nullptr, &prod));
-            tiles_in = tiles_d;
-            fold(L, STB_L_CQ_WG, STB_L_CQ_FOLD, d, f, whi, wlo, cb);
-            STB_TRY(lin(w.xs, d, whi, wlo, d, cb, STB_ACT_NONE, nullptr, w.q, none, d, nullptr, nullptr, &f));
-            Split Kx, vTx;
-            CrossDecodeKV Vd;
-            cross_ptrs(m, B, ckv, l, Kx, vTx, &Vd);
-            STB_TRY(decode_attn_cross(w.q, Vd, B, H, d, w.xpart, w.tickets, w.attn.hi, w.attn.lo, nullptr, st));
-            STB_TRY(lin(w.attn, d, W_HI(L, STB_L_COUT_W), W_LO(L, STB_L_COUT_W), d, W_F32(L, STB_L_COUT_B), STB_ACT_NONE, w.x,
-                        w.x, w.xs, d, nullptr, nullptr, &prod));
-            fold(L, STB_L_FC1_WG, STB_L_FC1_FOLD, 4 * d, f, whi, wlo, cb);
-            STB_TRY(lin(w.xs, d, whi, wlo, 4 * d, cb, STB_ACT_GELU, nullptr, nullptr, w.hid, 4 * d, nullptr, nullptr, &f));
-            STB_TRY(lin(w.hid, 4 * d, W_HI(L, STB_L_FC2_W), W_LO(L, STB_L_FC2_W), d, W_F32(L, STB_L_FC2_B), STB_ACT_NONE, w.x, w.x,
-                        w.xs, d, nullptr, nullptr, &prod));
-        }
-        DLFuse f = {w.stats, tiles_in, d, (const float*)t[STB_T_DEC_TOKEMB_FOLD][0], nullptr};
-        const float* cbv = (const float*)t[STB_T_DEC_TOKEMB_FOLD][0] + ((D.n_vocab + 3) & ~3);
-        STB_TRY(lin(w.xs, d, t[STB_T_DEC_TOKEMB_G][0], x3 ? t[STB_T_DEC_TOKEMB_G][1] : nullptr, D.n_vocab, cbv, STB_ACT_NONE, nullptr,
-                    logits, none, ld_logits, nullptr, nullptr, &f));
-        STB_TRY(bump_pos(pos, st));
-        return STB_OK;
-    }
     if (D.n_text_layer > 0)
         STB_TRY(layernorm(w.x, B, d, W_F32(m->dec[0], STB_L_ATTN_LN_G), W_F32(m->dec[0], STB_L_ATTN_LN_B), w.ln.hi, w.ln.lo, nullptr, st));
     else
@@ -597,8 +506,6 @@ extern "C" int stb_model_create(const stb_dims* dims, int precision, stb_model**
     stb_model* m = new stb_model();
     m->dims = *dims;
     m->prec = precision;
-    const char* e = getenv("STB_CONV_IM2COL");
-    m->conv_im2col = e && e[0] == '1';
     memset(m->t, 0, sizeof(m->t));
     m->enc.resize(dims->n_audio_layer);
     m->dec.resize(dims->n_text_layer);
@@ -657,7 +564,7 @@ static int check_weights(const stb_model* m, bool enc, bool dec) {
         STB_TRY(need(m->t[STB_T_DEC_LN_G], false, "dec.ln.g", -1));
         STB_TRY(need(m->t[STB_T_DEC_LN_B], false, "dec.ln.b", -1));
         for (size_t l = 0; l < m->dec.size(); ++l)
-            for (int id = 0; id < STB_L_QKV_WG; ++id) STB_TRY(need(m->dec[l].p[id], is_split(id), "dec.layer", (int)l));   // *_WG / *_FOLD are optional
+            for (int id = 0; id < STB_L_COUNT; ++id) STB_TRY(need(m->dec[l].p[id], is_split(id), "dec.layer", (int)l));   // a decoder layer uses every id
     }
     return STB_OK;
 }

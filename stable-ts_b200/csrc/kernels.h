@@ -31,7 +31,6 @@ int embed_tokens(const int32_t* tokens, long long n_tok, int M, int offset, int 
                  float* x, cudaStream_t st);
 int mel_repack(const float* mel, int B, int C, int T, __half* hi, __half* lo, cudaStream_t st);
 int zero_pad_rows(__half* hi, __half* lo, int B, int C, int T, cudaStream_t st);
-int im2col3(const __half* src, int B, int C, int Tin_pad, int Tout, int stride, __half* dst, cudaStream_t st);
 int capture_heads(const float* S, int B, int H, int M, long long ld, float* out, int n_sel, const CaptureList& list,
                   cudaStream_t st);
 
@@ -52,25 +51,12 @@ int gemv(const void* x_hi, const void* x_lo, int B, int K, const void* w_hi, con
          cudaStream_t st);
 // one Linear of the decode step in one launch: swapped wgmma GEMM, split-K across a thread-block cluster, partial tiles
 // reduced over distributed shared memory, fused bias / GELU / residual epilogue (decode_linear.cu)
-// fuse (nullable): LayerNorm folded into the Linear -- stats_in [tiles_in][B][2] partial (sum, sum of squares about the
-// tile's own mean) of the input rows (row_features values each) over 128-feature tiles, or over the whole row when
-// tiles_in == 1; wsum [n] row sums of the (W diag(gamma)) planes; stats_out [ceil(n / 128)][B][2]: the same partial
-// statistics of THIS Linear's output rows for the Linear after it
-struct DLFuse {
-    const float* stats_in;
-    int tiles_in;
-    int row_features;
-    const float* wsum;
-    float* stats_out;
-};
 int decode_linear(const void* x_hi, const void* x_lo, int B, int k, const void* w_hi, const void* w_lo, int n, const float* bias,
                   int act, const float* res, long long ld_res, float* out_f32, void* out_hi, void* out_lo, long long ld_out,
-                  const DLFuse* fuse, cudaStream_t st);
+                  cudaStream_t st);
 int decode_linear_split(int n, int k);
-// xs_hi / xs_lo / stats (nullable): split planes of x and its full-row (sum, sum of squares about the row mean) [1][B][2]
-// for a folded LayerNorm
 int embed_step(const int32_t* tokens, const int32_t* pos, const int32_t* seq_off, int n_pos, int B, int d, const float* emb,
-               const float* posemb, float* x, __half* xs_hi, __half* xs_lo, float* stats, cudaStream_t st);
+               const float* posemb, float* x, cudaStream_t st);
 int bump_pos(int32_t* pos, cudaStream_t st);
 
 }  // namespace stb

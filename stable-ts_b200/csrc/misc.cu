@@ -58,28 +58,6 @@ bool pdl_enabled(int kind) {
     return (v >> kind) & 1;
 }
 
-struct OptDef { const char* name; const char* env; int dflt; };
-static const OptDef g_opt_defs[OPT_COUNT] = {
-    // 1: the decode step folds every LayerNorm into the Linear that follows it (W diag(g) planes + row statistics from the
-    // producer's epilogue); needs the optional STB_L_*_WG / *_FOLD tensors, else the step runs its LayerNorm kernels.
-    // FP16X3 models only: an FP16 model's step ignores it
-    {"decode_fused_ln", "STB_DECODE_FUSED_LN", 0},
-};
-static int g_opt[OPT_COUNT];
-static bool g_opt_init = false;
-static void opt_init() {
-    if (g_opt_init) return;
-    for (int i = 0; i < OPT_COUNT; ++i) {
-        const char* e = getenv(g_opt_defs[i].env);
-        g_opt[i] = (e && e[0]) ? atoi(e) : g_opt_defs[i].dflt;
-    }
-    g_opt_init = true;
-}
-int option(Option o) {
-    opt_init();
-    return g_opt[o];
-}
-
 int& launch_priority() {
     static thread_local int p = 0;
     return p;
@@ -129,21 +107,7 @@ extern "C" int stb_axpby(float* y, const float* x, float a, float b, long long n
 }
 
 extern "C" const char* stb_last_error(void) { return stb::get_error(); }
-extern "C" int stb_abi_version(void) { return 6; }
-extern "C" int stb_set_option(const char* name, int value) {
-    STB_REQUIRE(name, "stb_set_option: null name");
-    stb::opt_init();
-    for (int i = 0; i < stb::OPT_COUNT; ++i)
-        if (strcmp(name, stb::g_opt_defs[i].name) == 0) { stb::g_opt[i] = value; return STB_OK; }
-    STB_REQUIRE(false, "stb_set_option: unknown option '%s'", name);
-    return STB_ERR_ARG;
-}
-extern "C" int stb_get_option(const char* name) {
-    stb::opt_init();
-    for (int i = 0; name && i < stb::OPT_COUNT; ++i)
-        if (strcmp(name, stb::g_opt_defs[i].name) == 0) return stb::g_opt[i];
-    return -1;
-}
+extern "C" int stb_abi_version(void) { return 7; }
 extern "C" unsigned long long stb_launch_count(void) { return stb::launches(); }
 
 extern "C" int stb_split_f16(const float* src, long long rows, int cols, long long src_ld, void* hi, void* lo,

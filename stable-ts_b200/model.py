@@ -54,27 +54,6 @@ def _split(w: torch.Tensor, want_lo: bool):
     return hi, lo
 
 
-def fold_layernorm_into_linear(w: torch.Tensor, bias: Optional[torch.Tensor], gamma: torch.Tensor, beta: torch.Tensor,
-                               want_lo: bool):
-    """LayerNorm (gamma, beta) folded into the Linear (w [n][d], bias) that follows it, for the decode step:
-    Linear(LayerNorm(x)) = rstd (W' x - mean rowsum(W')) + (W beta + bias) with W' = W diag(gamma).  Returns the split
-    planes (hi, lo or None) of W' and fold f32 [2][n rounded up to 4] = [row sums of exactly those planes | W beta + bias].
-    The sums are taken from the fp16 planes (what the tensor core multiplies), in float64, so that `acc - mean * rowsum`
-    cancels the way the GEMM adds."""
-    w = w.float()
-    wg = w * gamma.float()[None, :]
-    hi, lo = _split(wg, want_lo)
-    rows = hi.double().sum(1) if lo is None else (hi.double() + lo.double()).sum(1)
-    cb = w.double() @ beta.double()
-    if bias is not None:
-        cb = cb + bias.double()
-    n_pad = (rows.numel() + 3) // 4 * 4                   # both vectors start 16-byte aligned (V = 51866 is not a multiple of 4)
-    fold = torch.zeros(2, n_pad, dtype=torch.float32, device=rows.device)
-    fold[0, : rows.numel()] = rows.float()
-    fold[1, : rows.numel()] = cb.float()
-    return hi, lo, fold
-
-
 def mel_filterbank(n_mels: int) -> np.ndarray:
     """librosa-style Slaney mel filterbank (sr 16 kHz, n_fft 400), the matrix whisper ships as mel_filters.npz."""
     def hz2mel(f):
@@ -102,8 +81,7 @@ class B200Whisper(WhisperProtocol):
     protocol / ``detect_language``) that the unmodified reference code drives."""
 
     def __init__(self, dims, state_dict: Dict[str, torch.Tensor], device: Union[str, torch.device] = "cuda",
-                 precision: str = "fp16x3", alignment_heads: Optional[Sequence[Tuple[int, int]]] = None,
-                 fold_layernorm: bool = True):
+                 precision: str = "fp16x3", alignment_heads: Optional[Sequence[Tuple[int, int]]] = None):
         if not torch.cuda.is_available():
             raise RuntimeError("B200Whisper needs a CUDA device (there is no CPU fallback)")
         self.dims = ModelDimensions(**{k: int(getattr(dims, k)) for k in ModelDimensions.__dataclass_fields__})
@@ -111,10 +89,6 @@ class B200Whisper(WhisperProtocol):
         self.precision = precision
         self._prec = {"fp16x3": L.STB_PREC_FP16X3, "fp16": L.STB_PREC_FP16}[precision]
         self._want_lo = self._prec == L.STB_PREC_FP16X3
-        # also pack W diag(gamma) planes + fold vectors of the decoder linears that follow a LayerNorm: the decode step can
-        # then fold the LayerNorm into the Linear (option "decode_fused_ln"; +8 d^2 + V d weights, 1.9 GB at large-v3).
-        # fp16x3 only: the step never folds in fp16 (one plane of the raw row loses too much to rounding, engine.cu)
-        self.fold_layernorm = bool(fold_layernorm) and self._want_lo
         self._keep: List[torch.Tensor] = []
         self._ws: Dict[str, torch.Tensor] = {}
         self.graph_kernel_launches = 0     # kernels executed by CUDA-graph replays (the library counter only sees captures)
@@ -185,16 +159,6 @@ class B200Whisper(WhisperProtocol):
     def _set_f32(self, tid, is_dec, layer, w: torch.Tensor):
         self._set(tid, is_dec, layer, self._dev(w.float()))
 
-    def _set_folded(self, tid_w, tid_fold, is_dec, layer, w: torch.Tensor, bias: Optional[torch.Tensor], gamma: torch.Tensor,
-                    beta: torch.Tensor):
-        """LayerNorm (gamma, beta) folded into the Linear (w, bias) that follows it (STB_L_*_WG / *_FOLD), see
-        ``fold_layernorm_into_linear``."""
-        dev = self.device
-        hi, lo, fold = fold_layernorm_into_linear(w.to(dev), None if bias is None else bias.to(dev), gamma.to(dev), beta.to(dev),
-                                                  self._want_lo)
-        self._set(tid_w, is_dec, layer, self._dev(hi), self._dev(lo) if lo is not None else None)
-        self._set(tid_fold, is_dec, layer, self._dev(fold))
-
     def _pack(self, sd: Dict[str, torch.Tensor]):
         D = self.dims
         g = lambda k: sd[k].detach().float()
@@ -234,15 +198,6 @@ class B200Whisper(WhisperProtocol):
                 self._set_f32(B + L.L_CKV_B, 1, l, torch.cat([z, g(p + "cross_attn.value.bias")]))
                 self._set_split(B + L.L_COUT_W, 1, l, g(p + "cross_attn.out.weight"))
                 self._set_f32(B + L.L_COUT_B, 1, l, g(p + "cross_attn.out.bias"))
-                if self.fold_layernorm:
-                    self._set_folded(B + L.L_QKV_WG, B + L.L_QKV_FOLD, 1, l,
-                                     torch.cat([g(p + "attn.query.weight"), g(p + "attn.key.weight"), g(p + "attn.value.weight")]),
-                                     torch.cat([g(p + "attn.query.bias"), z, g(p + "attn.value.bias")]),
-                                     g(p + "attn_ln.weight"), g(p + "attn_ln.bias"))
-                    self._set_folded(B + L.L_CQ_WG, B + L.L_CQ_FOLD, 1, l, g(p + "cross_attn.query.weight"),
-                                     g(p + "cross_attn.query.bias"), g(p + "cross_attn_ln.weight"), g(p + "cross_attn_ln.bias"))
-                    self._set_folded(B + L.L_FC1_WG, B + L.L_FC1_FOLD, 1, l, g(p + "mlp.0.weight"), g(p + "mlp.0.bias"),
-                                     g(p + "mlp_ln.weight"), g(p + "mlp_ln.bias"))
 
         for l in range(D.n_audio_layer):
             block("encoder", 0, l, D.n_audio_state)
@@ -254,8 +209,6 @@ class B200Whisper(WhisperProtocol):
         self._set_f32(L.T_DEC_POS, 0, 0, g("decoder.positional_embedding"))
         self._set_f32(L.T_DEC_LN_G, 0, 0, g("decoder.ln.weight"))
         self._set_f32(L.T_DEC_LN_B, 0, 0, g("decoder.ln.bias"))
-        if self.fold_layernorm:
-            self._set_folded(L.T_DEC_TOKEMB_G, L.T_DEC_TOKEMB_FOLD, 0, 0, emb, None, g("decoder.ln.weight"), g("decoder.ln.bias"))
 
     def _frontend_tables(self):
         n = np.arange(400, dtype=np.float64)

@@ -263,41 +263,3 @@ def test_cross_attention_step_logits_match_float64():
     res, _ = decode_windows(gm2, tk2, gm2.encode(gm2.log_mel(audio.cuda()[None])), DecodingOptions(language="en", sample_len=16))
     assert res[0].tokens == ref.tokens and abs(res[0].avg_logprob - ref.avg_logprob) < 1e-3
 
-
-def test_layernorm_folded_into_the_step_linears():
-    """Option "decode_fused_ln": every LayerNorm of the decode step folded into the Linear after it (W diag(gamma) planes,
-    row statistics from the producer's epilogue) must reproduce the step with LayerNorm kernels: logits, tokens, log-probs."""
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from oracle import stable_path as SP
-    from oracle.whisper_ref.model import ModelDimensions
-    from stable_ts_b200 import _lib as L
-    from stable_ts_b200.decode import DecodingOptions, decode_windows
-    dims = ModelDimensions(n_mels=128, n_audio_ctx=1500, n_audio_state=1280, n_audio_head=20, n_audio_layer=1, n_vocab=51866,
-                           n_text_ctx=448, n_text_state=1280, n_text_head=20, n_text_layer=3)
-    W, model, gm, tk = _mk(dims, 29)
-    audios = torch.stack([SP.synth_audio(480000, seed=400 + i) for i in range(3)])
-    opt = DecodingOptions(sample_len=8)
-    default = L.get_option("decode_fused_ln")
-    try:
-        for rep in (7, 40):                                   # B = 21 (BN = 32) and B = 120 (BN = 128)
-            enc = gm.encode(gm.log_mel(audios.repeat(rep, 1).cuda()))
-            L.set_option("decode_fused_ln", 0)
-            r0, x0 = decode_windows(gm, tk, enc, opt, return_step_logits=True)
-            L.set_option("decode_fused_ln", 1)
-            r1, x1 = decode_windows(gm, tk, enc, opt, return_step_logits=True)
-            worst = 0.0
-            for a, b in zip(x0["step_logits"], x1["step_logits"]):
-                a, b = a.float().cpu(), b.float().cpu()
-                fin = a > -1e30
-                assert torch.equal(fin, b > -1e30)
-                worst = max(worst, ((a[fin] - b[fin]).abs().max() / a[fin].abs().max()).item())
-            print(f"B={3 * rep}: folded LayerNorm vs LayerNorm kernels, worst step-logit rel diff {worst:.2e}")
-            assert worst < 2e-5
-            for a, b in zip(r0, r1):
-                assert a.tokens == b.tokens and abs(a.avg_logprob - b.avg_logprob) < 1e-4
-            rg, _ = decode_windows(gm, tk, enc, opt)          # graph replay with the option on
-            for a, b in zip(r0, rg):
-                assert a.tokens == b.tokens
-    finally:
-        L.set_option("decode_fused_ln", default)

@@ -87,8 +87,8 @@ def bench_dtw(batches=(16, 64, 148)):
 
 def bench_step(windows=120, layers=4, s1=24, s2=72):
     """ms per KV-cached decode step of a large-v3-WIDTH model with `layers` decoder layers (cross K/V of 120 windows x 32
-    layers would not leave room for A/B runs), from the slope between two forced decodes of s1 and s2 steps (graph replay).
-    Use with STB_DECODE_FUSED_LN=1 to A/B the folded LayerNorm:  microbench.py step [windows] [layers]"""
+    layers would not leave room for A/B runs), from the slope between two forced decodes of s1 and s2 steps (graph replay):
+    microbench.py step [windows] [layers]"""
     import time
     from stable_ts_b200.api import random_state_dict
     from stable_ts_b200.decode import DecodingOptions, decode_windows
