@@ -251,21 +251,12 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_const
 template <int PASSES>
 static int launch_attention(const TmapVal (&tm)[6], AttnArgs& g, int n_batch, cudaStream_t st) {
     using Cfg = AttnCfg<PASSES>;
-    static bool attr_set[64] = {};    // per device ordinal
-    int dev = 0;
-    STB_CUDA_OK(cudaGetDevice(&dev));
-    if (dev < 0 || dev >= 64 || !attr_set[dev]) {
-        STB_CUDA_OK(cudaFuncSetAttribute(attention_tc_kernel<PASSES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM));
-        if (dev >= 0 && dev < 64) attr_set[dev] = true;
-    }
     dim3 grid(cdiv(g.Mq, AT_BQ), g.H, n_batch);
     const double zz = (double)n_batch * g.H;
     ProfScope ps("attention_tc", st, zz * ((double)g.Mq * 64 + 2.0 * g.Mk * 64) * 2.0 * Cfg::NPL + zz * g.Mq * 64.0 * 2.0 * Cfg::NPL,
                  zz * 4.0 * g.Mq * (double)g.Mk * 64);
-    attention_tc_kernel<PASSES><<<grid, AT_THREADS, Cfg::SMEM, st>>>(tm[0].map, tm[1].map, tm[2].map, tm[3].map, tm[4].map,
-                                                                      tm[5].map, g);
-    STB_LAUNCH_OK();
-    return STB_OK;
+    return launch(attention_tc_kernel<PASSES>, {grid, AT_THREADS, Cfg::SMEM, st}, tm[0].map, tm[1].map, tm[2].map, tm[3].map,
+                  tm[4].map, tm[5].map, g);
 }
 
 // q: rows Mq, k = 64; k: rows Mk, k = 64; vT: rows 64, k = keys (>= Mk, zero padded); out split [..][ld_out].

@@ -44,16 +44,6 @@ const char* get_error();
         }                                                                                              \
     } while (0)
 
-#define STB_LAUNCH_OK()                                                                                \
-    do {                                                                                               \
-        stb::count_launch();                                                                           \
-        cudaError_t e__ = cudaGetLastError();                                                          \
-        if (e__ != cudaSuccess) {                                                                      \
-            stb::set_error("%s:%d: kernel launch -> %s", __FILE__, __LINE__, cudaGetErrorString(e__));  \
-            return STB_ERR_CUDA;                                                                       \
-        }                                                                                              \
-    } while (0)
-
 #define STB_TRY(expr)                                                                                  \
     do {                                                                                               \
         int r__ = (expr);                                                                              \
@@ -70,49 +60,54 @@ struct ProfScope {
     int slot;
     cudaStream_t st;
 };
-void count_launch();   // every kernel launch of this library bumps the counter read by stb_launch_count()
-int sm_count();   // cached cudaDevAttrMultiProcessorCount of the current device
+int sm_count();   // cudaDevAttrMultiProcessorCount of the current device, cached per device ordinal
 
-#ifdef __CUDACC__
-// ---------------------------------------------------------------------------------------------------------
-// programmatic dependent launch (PDL): a kernel launched with `launch_pdl` may start while its predecessor in the
-// stream is still running; it must execute pdl_wait() before touching anything the predecessor writes.  pdl_trigger()
-// lets the NEXT kernel start early.  Both are no-ops for ordinary launches.
-// ---------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-
-bool pdl_enabled(int kind = 0);   // STB_PDL bit mask (misc.cu): kind 0 = ordinary kernels, 1 = decode_linear
 // launch priority of the kernels launched next by this host thread (cudaLaunchAttributePriority; 0 = the stream's own).
 // The decode step raises it for its latency-bound linear layers: under programmatic dependent launch the next kernel's CTAs
 // can become resident while the previous kernel's tail still runs, and the block scheduler then serves the higher-priority
 // CTAs first.  Not measured against priority 0.
 int& launch_priority();
 
+// ---------------------------------------------------------------------------------------------------------
+// Kernel launches.  Every kernel of this library is launched with stb::launch, which owns the launch policy (misc.cu):
+//  - programmatic dependent launch (PDL, `pdl`): the kernel may start while its predecessor in the stream is still
+//    running, so it must execute pdl_wait() before touching anything the predecessor writes; a kernel without that wait
+//    must not set `pdl`.  pdl_trigger() lets the NEXT kernel start early.  Both are no-ops for ordinary launches, and
+//    STB_PDL=0 turns PDL off for every launch.
+//  - the thread-block cluster (`cluster` = x-size; 0 = an ordinary launch, 1 = a cluster of one CTA);
+//  - launch_priority(), when it is not 0;
+//  - the opt-in to more dynamic shared memory than a kernel is allowed by default, per (kernel, device), and the
+//    largest shared-memory carveout when `max_carveout` is set;
+//  - one count per launch for stb_launch_count(), and the launch error check (the latched error is cleared).
+// ---------------------------------------------------------------------------------------------------------
+struct LaunchSpec {
+    dim3 grid, block;
+    size_t smem = 0;                            // dynamic shared memory, bytes
+    cudaStream_t stream = nullptr;
+    bool pdl = false;
+    unsigned cluster = 0;
+    bool max_carveout = false;
+    const char* file = __builtin_FILE();        // the call site, named by the launch error
+    int line = __builtin_LINE();
+};
+
+int launch_kernel(const void* kernel, const LaunchSpec& spec, void** args);
+// largest dynamic shared memory `kernel` can be launched with on the current device (the device's opt-in limit minus
+// the kernel's static shared memory)
+int max_dynamic_smem(const void* kernel, size_t* limit);
+
+// Returns STB_OK or STB_ERR_CUDA (message in stb_last_error).
 template <typename... KArgs, typename... Args>
-static inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = grid;
-    cfg.blockDim = block;
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[2];
-    int n = 0;
-    if (pdl_enabled()) {
-        attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[n].val.programmaticStreamSerializationAllowed = 1;
-        ++n;
-    }
-    if (launch_priority() != 0) {
-        attr[n].id = cudaLaunchAttributePriority;
-        attr[n].val.priority = launch_priority();
-        ++n;
-    }
-    cfg.attrs = attr;
-    cfg.numAttrs = n;
-    return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+static inline int launch(void (*kernel)(KArgs...), const LaunchSpec& spec, Args... args) {
+    return [&](KArgs... a) {
+        void* p[] = {(void*)&a...};
+        return launch_kernel((const void*)kernel, spec, p);
+    }(static_cast<KArgs>(args)...);
 }
+
+#ifdef __CUDACC__
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
 // ---------------------------------------------------------------------------------------------------------
 // warp helpers

@@ -578,11 +578,9 @@ extern "C" int stb_sample(float* logits, long long ld, int B, int V, int eot, in
     STB_REQUIRE(temperature >= 0.f && (temperature == 0.f || uniform_table != nullptr),
                 "stb_sample: temperature > 0 needs the table of uniform draws [table_rows][B]");
     stb::ProfScope ps("sample_greedy", (cudaStream_t)stream, (double)B * V * 4.0 * 3);
-    STB_CUDA_OK(stb::launch_pdl(stb::sample_greedy_kernel, dim3(B), dim3(1024), 0, (cudaStream_t)stream, logits, ld, V, eot, ts_begin,
-                                no_timestamps, suppress_mask, first_step_mask, ts_mask, ts_mask_stride, max_initial_ts, apply_ts_rules, forced_table,
-                                states, next_out, token_table, argmax_table, table_rows, temperature, uniform_table, sample_cap));
-    STB_LAUNCH_OK();
-    return STB_OK;
+    return stb::launch(stb::sample_greedy_kernel, {dim3(B), dim3(1024), 0, (cudaStream_t)stream, /*pdl=*/true}, logits, ld, V, eot,
+                       ts_begin, no_timestamps, suppress_mask, first_step_mask, ts_mask, ts_mask_stride, max_initial_ts, apply_ts_rules,
+                       forced_table, states, next_out, token_table, argmax_table, table_rows, temperature, uniform_table, sample_cap);
 }
 
 extern "C" int stb_sample_greedy(float* logits, long long ld, int B, int V, int eot, int ts_begin, int no_timestamps,
@@ -598,21 +596,11 @@ namespace stb {
 int decode_attn_self(const float* qkv, float* Kc, float* Vc, int B, int H, int d, int ctx, const int32_t* pos,
                      const int32_t* seq_off, __half* oh, __half* ol, float* of, cudaStream_t st) {
     ProfScope ps("decode_self_attn", st);
-    STB_CUDA_OK(launch_pdl(decode_self_attn_kernel, dim3(H, B), dim3(128), 0, st, qkv, Kc, Vc, d, ctx, pos, seq_off, oh, ol, of));
-    STB_LAUNCH_OK();
-    return STB_OK;
+    return launch(decode_self_attn_kernel, {dim3(H, B), dim3(128), 0, st, /*pdl=*/true}, qkv, Kc, Vc, d, ctx, pos, seq_off, oh, ol, of);
 }
 int decode_attn_cross(const float* q, const CrossDecodeKV& kv, int B, int H, int d, float* partial, int* tickets, __half* oh,
                       __half* ol, float* of, cudaStream_t st) {
     ProfScope ps("decode_cross_attn", st, (double)B * H * 2.0 * STB_N_AUDIO_CTX * 64 * 2.0);
-    static bool attr_set[64] = {};                          // per device ordinal
-    int dev = 0;
-    STB_CUDA_OK(cudaGetDevice(&dev));
-    if (dev >= 0 && dev < 64 && !attr_set[dev]) {
-        STB_CUDA_OK(cudaFuncSetAttribute(decode_cross_attn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, XT_SMEM));
-        STB_CUDA_OK(cudaFuncSetAttribute(decode_cross_attn_tc_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
-        attr_set[dev] = true;
-    }
     const int T = (int)STB_N_AUDIO_CTX;
     TmapVal tk, tv;
     STB_TRY(make_tmap(kv.k_hi, T, 64, H, B, 64, (long long)T * 64, (long long)H * T * 64, XT_KEYS, &tk));
@@ -622,28 +610,21 @@ int decode_attn_cross(const float* q, const CrossDecodeKV& kv, int B, int H, int
         STB_REQUIRE(tk.perm[i] == tv.perm[i], "decode_attn_cross: K / V tensor maps disagree");
         perm.p[i] = tk.perm[i];
     }
-    STB_CUDA_OK(launch_pdl(decode_cross_attn_tc_kernel, dim3(XS, H, B), dim3(128), (size_t)XT_SMEM, st, tk.map, tv.map, perm, q, d,
-                           T, partial, tickets, oh, ol, of));
-    STB_LAUNCH_OK();
-    return STB_OK;
+    return launch(decode_cross_attn_tc_kernel,
+                  {dim3(XS, H, B), dim3(128), (size_t)XT_SMEM, st, /*pdl=*/true, /*cluster=*/0, /*max_carveout=*/true}, tk.map, tv.map,
+                  perm, q, d, T, partial, tickets, oh, ol, of);
 }
 int decode_cross_splits() { return XS; }
 int v_headmajor(const __half* vT_hi, int BH, int T, int Tp, __half* v_hi, cudaStream_t st) {
     ProfScope ps("v_headmajor", st, (double)BH * T * 64 * 4.0);
-    v_headmajor_kernel<<<dim3(cdiv(T, 64), BH), 256, 0, st>>>(vT_hi, T, Tp, v_hi);
-    STB_LAUNCH_OK();
-    return STB_OK;
+    return launch(v_headmajor_kernel, {dim3(cdiv(T, 64), BH), 256, 0, st}, vT_hi, T, Tp, v_hi);
 }
 int embed_step(const int32_t* tokens, const int32_t* pos, const int32_t* seq_off, int n_pos, int B, int d, const float* emb,
                const float* posemb, float* x, cudaStream_t st) {
-    STB_CUDA_OK(launch_pdl(embed_step_kernel, dim3(B), dim3(128), 0, st, tokens, pos, seq_off, n_pos, d, emb, posemb, x));
-    STB_LAUNCH_OK();
-    return STB_OK;
+    return launch(embed_step_kernel, {dim3(B), dim3(128), 0, st, /*pdl=*/true}, tokens, pos, seq_off, n_pos, d, emb, posemb, x);
 }
 int bump_pos(int32_t* pos, cudaStream_t st) {
-    STB_CUDA_OK(launch_pdl(bump_pos_kernel, dim3(1), dim3(1), 0, st, pos));
-    STB_LAUNCH_OK();
-    return STB_OK;
+    return launch(bump_pos_kernel, {dim3(1), dim3(1), 0, st, /*pdl=*/true}, pos);
 }
 }  // namespace stb
 

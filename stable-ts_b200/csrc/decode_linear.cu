@@ -304,47 +304,13 @@ template <int BN, int PASSES>
 static int launch_dl(const TmapVal& wh, const TmapVal& wl, const TmapVal& xh, const TmapVal& xl, const DLArgs& g, int split,
                      cudaStream_t st) {
     using Cfg = DLCfg<BN, PASSES>;
-    static bool attr_set[64] = {};
-    int dev = 0;
-    STB_CUDA_OK(cudaGetDevice(&dev));
-    if (dev >= 0 && dev < 64 && !attr_set[dev]) {
-        STB_CUDA_OK(cudaFuncSetAttribute(decode_linear_kernel<BN, PASSES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM));
-        attr_set[dev] = true;
-    }
     const int mt = cdiv(g.n, 128);
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3((unsigned)(mt * split));
-    cfg.blockDim = dim3(DL_THREADS);
-    cfg.dynamicSmemBytes = Cfg::SMEM;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[3];
-    int na = 0;
-    attr[na].id = cudaLaunchAttributeClusterDimension;
-    attr[na].val.clusterDim.x = (unsigned)split;
-    attr[na].val.clusterDim.y = 1;
-    attr[na].val.clusterDim.z = 1;
-    ++na;
-    if (pdl_enabled(1)) {
-        attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[na].val.programmaticStreamSerializationAllowed = 1;
-        ++na;
-    }
-    if (launch_priority() != 0) {
-        attr[na].id = cudaLaunchAttributePriority;
-        attr[na].val.priority = launch_priority();
-        ++na;
-    }
-    cfg.attrs = attr;
-    cfg.numAttrs = na;
-    {
-        const double wbytes = (double)g.n * g.kb_total * 64 * 2.0 * Cfg::NPL;
-        ProfScope ps("decode_linear", st, wbytes + (double)g.B * g.kb_total * 64 * 2.0 * Cfg::NPL + (double)g.B * g.n * 4.0,
-                     2.0 * g.n * (double)g.B * g.kb_total * 64);
-        STB_CUDA_OK(cudaLaunchKernelEx(&cfg, decode_linear_kernel<BN, PASSES>, wh.map, wl.map, xh.map, xl.map, g));
-    }
-    STB_LAUNCH_OK();
-    return STB_OK;
+    const double wbytes = (double)g.n * g.kb_total * 64 * 2.0 * Cfg::NPL;
+    ProfScope ps("decode_linear", st, wbytes + (double)g.B * g.kb_total * 64 * 2.0 * Cfg::NPL + (double)g.B * g.n * 4.0,
+                 2.0 * g.n * (double)g.B * g.kb_total * 64);
+    return launch(decode_linear_kernel<BN, PASSES>,
+                  {dim3((unsigned)(mt * split)), dim3(DL_THREADS), Cfg::SMEM, st, /*pdl=*/true, /*cluster=*/(unsigned)split}, wh.map,
+                  wl.map, xh.map, xl.map, g);
 }
 
 // out[B][n] = epilogue(x[B][k] . W[n][k]^T); x / W split-fp16 planes, K-major; B <= 128; k a multiple of 64.

@@ -249,29 +249,14 @@ extern "C" int stb_dtw(const float* x, int B, int R, int F, long long ldx, int n
     STB_REQUIRE(B >= 1 && R >= 1 && F >= 1 && R <= stb::DTW_MAX_ROWS && F <= 1504 && ldx >= F,
                 "stb_dtw: unsupported shape B=%d R=%d F=%d ld=%lld (R<=%d, F<=1504)", B, R, F, ldx, stb::DTW_MAX_ROWS);
     const size_t smem = stb::dtw_smem(R, F);
-    static size_t max_dyn_dev[64] = {};  // per device ordinal: opt-in limit minus the kernel's static shared memory
-    int dev = 0;
-    STB_CUDA_OK(cudaGetDevice(&dev));
-    STB_REQUIRE(dev >= 0 && dev < 64, "stb_dtw: device ordinal %d out of range", dev);
-    if (max_dyn_dev[dev] == 0) {
-        int optin = 0;
-        cudaFuncAttributes fa;
-        STB_CUDA_OK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-        STB_CUDA_OK(cudaFuncGetAttributes(&fa, stb::dtw_kernel));
-        const size_t lim = (size_t)optin - fa.sharedSizeBytes;
-        STB_CUDA_OK(cudaFuncSetAttribute(stb::dtw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lim));
-        max_dyn_dev[dev] = lim;
-    }
-    const size_t max_dyn = max_dyn_dev[dev];
+    size_t max_dyn = 0;
+    STB_TRY(stb::max_dynamic_smem((const void*)stb::dtw_kernel, &max_dyn));
     STB_REQUIRE(smem <= max_dyn, "stb_dtw: trace needs %zu B of shared memory (limit %zu)", smem, max_dyn);
     const int NW = (R + 31) / 32;
     const int Rpad = NW * 32;
     cudaStream_t st = (cudaStream_t)stream;
     stb::ProfScope ps("dtw(+skew)", st, (double)B * R * F * 4.0 * 3, (double)B * R * F);
     STB_CUDA_OK(cudaMemsetAsync(ws, 0, stb_dtw_ws_bytes(B, R, F), st));      // zero border (t - (r&31) outside [0,F))
-    stb::dtw_skew_kernel<<<dim3(stb::cdiv(F, 32), NW, B), 256, 0, st>>>(x, R, F, ldx, Rpad, negate, (float*)ws);
-    STB_LAUNCH_OK();
-    stb::dtw_kernel<<<B, NW * 32, smem, st>>>((const float*)ws, R, F, Rpad, jumps, path, path_len);
-    STB_LAUNCH_OK();
-    return STB_OK;
+    STB_TRY(stb::launch(stb::dtw_skew_kernel, {dim3(stb::cdiv(F, 32), NW, B), 256, 0, st}, x, R, F, ldx, Rpad, negate, (float*)ws));
+    return stb::launch(stb::dtw_kernel, {B, NW * 32, smem, st}, (const float*)ws, R, F, Rpad, jumps, path, path_len);
 }

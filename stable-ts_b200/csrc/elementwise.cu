@@ -67,9 +67,7 @@ int layernorm(const float* x, long long rows, int d, const float* gamma, const f
     STB_REQUIRE(d % 128 == 0 && d <= 1280, "layernorm: d=%d must be a multiple of 128 and <= 1280", d);
     if (rows == 0) return STB_OK;
     ProfScope ps("layernorm", st, (double)rows * d * (4.0 + (hi ? 2.0 : 0.0) + (lo ? 2.0 : 0.0) + (out_f32 ? 4.0 : 0.0)));
-    STB_CUDA_OK(launch_pdl(layernorm_kernel, dim3(cdiv(rows, 8)), dim3(256), 0, st, x, rows, d, gamma, beta, hi, lo, out_f32));
-    STB_LAUNCH_OK();
-    return STB_OK;
+    return launch(layernorm_kernel, {dim3(cdiv(rows, 8)), dim3(256), 0, st, /*pdl=*/true}, x, rows, d, gamma, beta, hi, lo, out_f32);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -123,9 +121,7 @@ int softmax_rows(const float* S, long long n_rows, int n_cols, long long ld_s, i
                 SM_MAXV * 32);
     if (n_rows == 0) return STB_OK;
     ProfScope ps("softmax", st, (double)n_rows * n_cols * 4.0 + (double)n_rows * ld_p * 2.0 * (lo ? 2 : 1));
-    softmax_kernel<<<cdiv(n_rows, 8), 256, 0, st>>>(S, n_rows, n_cols, ld_s, rows_per_slice, causal, hi, lo, ld_p);
-    STB_LAUNCH_OK();
-    return STB_OK;
+    return launch(softmax_kernel, {cdiv(n_rows, 8), 256, 0, st}, S, n_rows, n_cols, ld_s, rows_per_slice, causal, hi, lo, ld_p);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -148,9 +144,7 @@ __global__ void embed_kernel(const int32_t* __restrict__ tokens, long long n_tok
 int embed_tokens(const int32_t* tokens, long long n_tok, int M, int offset, int d, const float* emb, const float* pos,
                  float* x, cudaStream_t st) {
     if (n_tok == 0) return STB_OK;
-    embed_kernel<<<(unsigned)n_tok, 128, 0, st>>>(tokens, n_tok, M, offset, d, emb, pos, x);
-    STB_LAUNCH_OK();
-    return STB_OK;
+    return launch(embed_kernel, {(unsigned)n_tok, 128, 0, st}, tokens, n_tok, M, offset, d, emb, pos, x);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -191,9 +185,7 @@ __global__ void __launch_bounds__(256) mel_repack_kernel(const float* __restrict
 
 int mel_repack(const float* mel, int B, int C, int T, __half* hi, __half* lo, cudaStream_t st) {
     dim3 grid(cdiv(T, 32), cdiv(C, 32), B);
-    mel_repack_kernel<<<grid, 256, 0, st>>>(mel, C, T, hi, lo);
-    STB_LAUNCH_OK();
-    return STB_OK;
+    return launch(mel_repack_kernel, {grid, 256, 0, st}, mel, C, T, hi, lo);
 }
 
 // zero the padding rows (0 and T+1) of a time-major [B][T+2][C] split buffer
@@ -207,9 +199,7 @@ __global__ void zero_pad_rows_kernel(__half* hi, __half* lo, int C, int T) {
     }
 }
 int zero_pad_rows(__half* hi, __half* lo, int B, int C, int T, cudaStream_t st) {
-    zero_pad_rows_kernel<<<B, 256, 0, st>>>(hi, lo, C, T);
-    STB_LAUNCH_OK();
-    return STB_OK;
+    return launch(zero_pad_rows_kernel, {B, 256, 0, st}, hi, lo, C, T);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -231,9 +221,7 @@ int capture_heads(const float* S, int B, int H, int M, long long ld, float* out,
     const long long slice = (long long)M * ld;
     STB_REQUIRE(slice % 4 == 0, "capture: slice not a multiple of 4 floats");
     dim3 grid(min(cdiv(slice / 4, 256), 64), list.count, B);
-    capture_kernel<<<grid, 256, 0, st>>>(S, H, slice, out, n_sel, list);
-    STB_LAUNCH_OK();
-    return STB_OK;
+    return launch(capture_kernel, {grid, 256, 0, st}, S, H, slice, out, n_sel, list);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -315,9 +303,7 @@ extern "C" int stb_softmax_probs(const float* logits, long long ld, int n_rows, 
     STB_REQUIRE(logits && out && n_classes > 0 && ld >= n_classes && ld_out >= n_classes, "stb_softmax_probs: bad arguments");
     if (n_rows == 0) return STB_OK;
     stb::ProfScope ps("softmax_probs", (cudaStream_t)stream, (double)n_rows * n_classes * 8.0);
-    stb::softmax_probs_kernel<<<n_rows, 512, 0, (cudaStream_t)stream>>>(logits, ld, n_classes, out, ld_out);
-    STB_LAUNCH_OK();
-    return STB_OK;
+    return stb::launch(stb::softmax_probs_kernel, {n_rows, 512, 0, (cudaStream_t)stream}, logits, ld, n_classes, out, ld_out);
 }
 
 extern "C" int stb_token_probs(const float* logits, long long ld, int n_rows, int n_classes, const int32_t* targets,
@@ -325,9 +311,8 @@ extern "C" int stb_token_probs(const float* logits, long long ld, int n_rows, in
     STB_REQUIRE(logits && targets && prob_out && n_classes > 0 && ld >= n_classes, "stb_token_probs: bad arguments");
     if (n_rows == 0) return STB_OK;
     stb::ProfScope ps("token_prob", (cudaStream_t)stream, (double)n_rows * n_classes * 4.0);
-    stb::token_prob_kernel<<<n_rows, 512, 0, (cudaStream_t)stream>>>(logits, ld, n_classes, targets, prob_out, rank_out);
-    STB_LAUNCH_OK();
-    return STB_OK;
+    return stb::launch(stb::token_prob_kernel, {n_rows, 512, 0, (cudaStream_t)stream}, logits, ld, n_classes, targets, prob_out,
+                       rank_out);
 }
 
 // ---------------------------------------------------------------------------------------------------------

@@ -381,14 +381,6 @@ template <int BN, int PASSES>
 static int launch_gemm(const TmapVal& ah, const TmapVal& al, const TmapVal& bh, const TmapVal& bl, GemmArgs& g,
                        int n_batch, cudaStream_t st) {
     using Cfg = GemmCfg<BN, PASSES>;
-    static bool attr_set[64] = {};    // per instantiation and device ordinal (function attributes are per device)
-    int dev = 0;
-    STB_CUDA_OK(cudaGetDevice(&dev));
-    if (dev < 0 || dev >= 64 || !attr_set[dev]) {
-        STB_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<BN, PASSES>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)Cfg::SMEM));
-        if (dev >= 0 && dev < 64) attr_set[dev] = true;
-    }
     for (int i = 0; i < 3; ++i) {
         g.permA[i] = ah.perm[i];
         g.permB[i] = bh.perm[i];
@@ -396,16 +388,12 @@ static int launch_gemm(const TmapVal& ah, const TmapVal& al, const TmapVal& bh, 
     g.Z = n_batch * g.H;
     const long long num_tiles = (long long)cdiv(g.N, BN) * cdiv(g.M, 128) * g.Z;
     dim3 grid((unsigned)(num_tiles < sm_count() ? num_tiles : sm_count()));     // persistent: one CTA per SM
-    {
-        // algorithmic FLOPs of ONE fp32-grade GEMM (not x PASSES); bytes: operands once + output once
-        const double zz = (double)n_batch * g.H;
-        ProfScope ps("gemm_tc", st, zz * ((double)g.M * g.K + (double)g.N * g.K) * 2.0 * Cfg::NPL + zz * (double)g.M * g.N * 4.0,
-                     2.0 * g.M * (double)g.N * g.K * zz);
-        STB_CUDA_OK(launch_pdl(gemm_tc_kernel<BN, PASSES>, grid, dim3(GEMM_THREADS), (size_t)Cfg::SMEM, st, ah.map, al.map, bh.map,
-                               bl.map, g));
-    }
-    STB_LAUNCH_OK();
-    return STB_OK;
+    // algorithmic FLOPs of ONE fp32-grade GEMM (not x PASSES); bytes: operands once + output once
+    const double zz = (double)n_batch * g.H;
+    ProfScope ps("gemm_tc", st, zz * ((double)g.M * g.K + (double)g.N * g.K) * 2.0 * Cfg::NPL + zz * (double)g.M * g.N * 4.0,
+                 2.0 * g.M * (double)g.N * g.K * zz);
+    return launch(gemm_tc_kernel<BN, PASSES>, {grid, dim3(GEMM_THREADS), (size_t)Cfg::SMEM, st, /*pdl=*/true}, ah.map, al.map,
+                  bh.map, bl.map, g);
 }
 
 int gemm(const stb_operand& A, const stb_operand& B, int n_batch, int n_head, const stb_epilogue& ep, cudaStream_t st) {

@@ -165,18 +165,10 @@ int gemv(const void* x_hi, const void* x_lo, int B, int K, const void* w_hi, con
     STB_REQUIRE(B >= 1 && B <= 64 && K % 32 == 0 && K >= 32, "gemv: unsupported shape B=%d K=%d", B, K);
     const int kc = K < GM_KC ? K : GM_KC;
     const size_t smem = (size_t)32 * (kc * 2 + 64) + GM_WARPS * 128 * sizeof(float);
-    static size_t configured = 0;
-    if (smem > 48 * 1024 && smem > configured) {
-        const size_t want = (size_t)32 * (GM_KC * 2 + 64) + GM_WARPS * 128 * sizeof(float);
-        STB_CUDA_OK(cudaFuncSetAttribute(gemv_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)want));
-        configured = want;
-    }
     ProfScope ps("gemv_mma", st, (double)N * K * 2.0 * (w_lo ? 2 : 1) + (double)B * K * 4.0 + (double)B * N * 4.0, 2.0 * B * (double)N * K);
-    STB_CUDA_OK(launch_pdl(gemv_mma_kernel, dim3(cdiv(N, 8)), dim3(GM_WARPS * 32), smem, st, (const __half*)x_hi,
-                           (const __half*)x_lo, B, K, (const __half*)w_hi, (const __half*)w_lo, N, bias, act, res, ld_res,
-                           out_f32, (__half*)out_hi, (__half*)out_lo, ld_out));
-    STB_LAUNCH_OK();
-    return STB_OK;
+    return launch(gemv_mma_kernel, {dim3(cdiv(N, 8)), dim3(GM_WARPS * 32), smem, st, /*pdl=*/true}, (const __half*)x_hi,
+                  (const __half*)x_lo, B, K, (const __half*)w_hi, (const __half*)w_lo, N, bias, act, res, ld_res, out_f32,
+                  (__half*)out_hi, (__half*)out_lo, ld_out);
 }
 
 }  // namespace stb

@@ -131,11 +131,8 @@ extern "C" int stb_logmel(const float* audio, int B, int n_samples, int padded_s
     cudaStream_t st = (cudaStream_t)stream;
     // every CTA writes its max (-inf when it holds no valid frame) so the workspace needs no initialisation
     stb::ProfScope ps("logmel(2 kernels)", st, (double)B * (n_samples * 4.0 + n_mels * 3000 * 4.0));
-    stb::logmel_kernel<<<dim3(blocks, B), stb::LM_THREADS, 0, st>>>(audio, n_samples, padded_samples, n_frames, n_mels,
-                                                                     filters, window, dft_table, mel_out, (float*)ws);
-    STB_LAUNCH_OK();
-    stb::logmel_finalize_kernel<<<dim3(64, B), 256, 0, st>>>(mel_out, n_mels, n_frames, (const float*)ws, blocks, B,
-                                                            batch_global_max);
-    STB_LAUNCH_OK();
-    return STB_OK;
+    STB_TRY(stb::launch(stb::logmel_kernel, {dim3(blocks, B), stb::LM_THREADS, 0, st}, audio, n_samples, padded_samples, n_frames,
+                        n_mels, filters, window, dft_table, mel_out, (float*)ws));
+    return stb::launch(stb::logmel_finalize_kernel, {dim3(64, B), 256, 0, st}, mel_out, n_mels, n_frames, (const float*)ws, blocks,
+                       B, batch_global_max);
 }

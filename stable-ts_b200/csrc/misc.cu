@@ -1,10 +1,11 @@
-// Error plumbing, device attributes and small utility kernels shared by the C ABI.
+// Error plumbing, the kernel launch helper with its per-device state, and small utility kernels shared by the C ABI.
 #include <stdarg.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
 
 #include <map>
+#include <mutex>
 #include <string>
 #include <vector>
 
@@ -24,7 +25,6 @@ void set_error(const char* fmt, ...) {
 const char* get_error() { return g_err; }
 
 static unsigned long long g_launches = 0;
-void count_launch() { ++g_launches; }
 unsigned long long launches() { return g_launches; }
 
 // ---- event profiler ----
@@ -47,15 +47,16 @@ ProfScope::~ProfScope() {
     if (slot >= 0) cudaEventRecord(g_prof[slot].e1, st);
 }
 
-// STB_PDL: bit 0 = programmatic dependent launch for the ordinary kernels (launch_pdl), bit 1 = for the cluster kernel of
-// the decode-step linears.  Default 3 (both); 0 disables it everywhere (the in-kernel griddepcontrol instructions are then no-ops).
-bool pdl_enabled(int kind) {
-    static int v = -1;
-    if (v < 0) {
+// ---- launch policy (common.cuh: LaunchSpec) ----
+
+// STB_PDL=0 turns programmatic dependent launch off for every kernel (the in-kernel griddepcontrol instructions are then
+// no-ops); unset or any other value leaves it on.
+static bool pdl_enabled() {
+    static const bool on = [] {
         const char* e = getenv("STB_PDL");
-        v = (e && e[0]) ? atoi(e) : 3;
-    }
-    return (v >> kind) & 1;
+        return !(e && strcmp(e, "0") == 0);
+    }();
+    return on;
 }
 
 int& launch_priority() {
@@ -63,14 +64,104 @@ int& launch_priority() {
     return p;
 }
 
+// Per-device state.  Function attributes and SM counts belong to a device, and a process may drive models on several.
+struct FuncSmem {
+    size_t opted;      // dynamic shared memory the kernel may currently be launched with
+    size_t limit;      // the device's opt-in limit minus the kernel's static shared memory
+    bool carveout;     // the largest carveout is set
+};
+static std::mutex g_dev_mu;
+static std::map<int, int> g_sms;                                     // device ordinal -> multiprocessor count
+static std::map<std::pair<const void*, int>, FuncSmem> g_smem;       // (kernel, device ordinal) -> shared memory
+
 int sm_count() {
-    static int n = 0;
-    if (n == 0) {
-        int dev = 0;
-        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
-            n = 132;
-    }
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+    std::lock_guard<std::mutex> lk(g_dev_mu);
+    int& n = g_sms[dev];
+    if (n == 0 && cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) n = 132;
     return n;
+}
+
+// the entry of `kernel` on the current device; the caller holds g_dev_mu
+static int func_smem(const void* kernel, FuncSmem** out) {
+    int dev = 0;
+    STB_CUDA_OK(cudaGetDevice(&dev));
+    auto it = g_smem.find({kernel, dev});
+    if (it == g_smem.end()) {
+        cudaFuncAttributes fa;
+        int optin = 0;
+        STB_CUDA_OK(cudaFuncGetAttributes(&fa, kernel));
+        STB_CUDA_OK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+        const FuncSmem f = {(size_t)fa.maxDynamicSharedSizeBytes, (size_t)optin - fa.sharedSizeBytes, false};
+        it = g_smem.emplace(std::make_pair(kernel, dev), f).first;
+    }
+    *out = &it->second;
+    return STB_OK;
+}
+
+int max_dynamic_smem(const void* kernel, size_t* limit) {
+    std::lock_guard<std::mutex> lk(g_dev_mu);
+    FuncSmem* f = nullptr;
+    STB_TRY(func_smem(kernel, &f));
+    *limit = f->limit;
+    return STB_OK;
+}
+
+static int opt_in_smem(const void* kernel, size_t smem, bool max_carveout) {
+    std::lock_guard<std::mutex> lk(g_dev_mu);
+    FuncSmem* f = nullptr;
+    STB_TRY(func_smem(kernel, &f));
+    if (smem > f->opted) {
+        STB_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        f->opted = smem;
+    }
+    if (max_carveout && !f->carveout) {
+        STB_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
+        f->carveout = true;
+    }
+    return STB_OK;
+}
+
+int launch_kernel(const void* kernel, const LaunchSpec& s, void** args) {
+    if (s.smem > 0 || s.max_carveout) STB_TRY(opt_in_smem(kernel, s.smem, s.max_carveout));
+    cudaLaunchConfig_t cfg;
+    memset(&cfg, 0, sizeof(cfg));
+    cfg.gridDim = s.grid;
+    cfg.blockDim = s.block;
+    cfg.dynamicSmemBytes = s.smem;
+    cfg.stream = s.stream;
+    cudaLaunchAttribute attr[3];
+    unsigned n = 0;
+    if (s.cluster > 0) {
+        attr[n].id = cudaLaunchAttributeClusterDimension;
+        attr[n].val.clusterDim.x = s.cluster;
+        attr[n].val.clusterDim.y = 1;
+        attr[n].val.clusterDim.z = 1;
+        ++n;
+    }
+    if (s.pdl && pdl_enabled()) {
+        attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        attr[n].val.programmaticStreamSerializationAllowed = 1;
+        ++n;
+    }
+    const int priority = launch_priority();
+    if (priority != 0) {
+        attr[n].id = cudaLaunchAttributePriority;
+        attr[n].val.priority = priority;
+        ++n;
+    }
+    cfg.attrs = attr;
+    cfg.numAttrs = n;
+    cudaError_t e = cudaLaunchKernelExC(&cfg, kernel, args);
+    ++g_launches;
+    const cudaError_t latched = cudaGetLastError();      // also clears the launch's own error
+    if (e == cudaSuccess) e = latched;
+    if (e != cudaSuccess) {
+        set_error("%s:%d: kernel launch -> %s", s.file, s.line, cudaGetErrorString(e));
+        return STB_ERR_CUDA;
+    }
+    return STB_OK;
 }
 
 // fp32 [rows][cols] -> fp16 hi (+ lo) planes.  8 elements per thread, 128-bit loads/stores where aligned.
@@ -101,9 +192,7 @@ extern "C" int stb_axpby(float* y, const float* x, float a, float b, long long n
     if (n == 0) return STB_OK;
     const int cap = stb::sm_count() * 8;
     const int grid = (int)((n + 255) / 256 < cap ? (n + 255) / 256 : cap);
-    stb::axpby_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(y, x, a, b, n);
-    STB_LAUNCH_OK();
-    return STB_OK;
+    return stb::launch(stb::axpby_kernel, {grid, 256, 0, (cudaStream_t)stream}, y, x, a, b, n);
 }
 
 extern "C" const char* stb_last_error(void) { return stb::get_error(); }
@@ -118,9 +207,8 @@ extern "C" int stb_split_f16(const float* src, long long rows, int cols, long lo
     int blocks = (int)((total + 255) / 256);
     const int cap = stb::sm_count() * 16;
     if (blocks > cap) blocks = cap;
-    stb::split_f16_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(src, rows, cols, src_ld, (__half*)hi, (__half*)lo, dst_ld);
-    STB_LAUNCH_OK();
-    return STB_OK;
+    return stb::launch(stb::split_f16_kernel, {blocks, 256, 0, (cudaStream_t)stream}, src, rows, cols, src_ld, (__half*)hi,
+                       (__half*)lo, dst_ld);
 }
 
 extern "C" void stb_prof_enable(int on) { stb::g_prof_on = on != 0; }

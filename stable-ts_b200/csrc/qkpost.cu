@@ -122,13 +122,10 @@ extern "C" int stb_qk_postprocess(const float* qk, int B, int A, int M, long lon
     cudaStream_t st = (cudaStream_t)stream;
     const long long n_rows = (long long)B * A * R;
     stb::ProfScope ps("qk_postprocess(3 kernels)", st, (double)B * A * R * F * 4.0 + (double)B * R * F * 4.0);
-    stb::qk_softmax_kernel<<<stb::cdiv(n_rows, 8), 256, 0, st>>>(qk, n_rows, M, ldq, S, R, F, qk_scale, W, Fp);
-    STB_LAUNCH_OK();
-    stb::qk_znorm_kernel<<<dim3(stb::cdiv(F, 128), B * A), 128, 0, st>>>(W, R, F, Fp);
-    STB_LAUNCH_OK();
-    stb::qk_median_mean_kernel<<<dim3(stb::cdiv(F, 128), R, B), 128, 0, st>>>(W, A, R, F, Fp, medfilt_width, matrix, ldm);
-    STB_LAUNCH_OK();
-    return STB_OK;
+    STB_TRY(stb::launch(stb::qk_softmax_kernel, {stb::cdiv(n_rows, 8), 256, 0, st}, qk, n_rows, M, ldq, S, R, F, qk_scale, W, Fp));
+    STB_TRY(stb::launch(stb::qk_znorm_kernel, {dim3(stb::cdiv(F, 128), B * A), 128, 0, st}, W, R, F, Fp));
+    return stb::launch(stb::qk_median_mean_kernel, {dim3(stb::cdiv(F, 128), R, B), 128, 0, st}, W, A, R, F, Fp, medfilt_width, matrix,
+                       ldm);
 }
 
 // =========================================================================================================
@@ -369,21 +366,14 @@ extern "C" int stb_qk_postprocess_dynamic(const float* qk, int B, int LH, int M,
     int32_t* table = (int32_t*)(scores + (size_t)B * LH * R);   // [B][count][R]
     const long long n_rows = (long long)B * LH * R;
     stb::ProfScope ps("qk_postprocess_dynamic", st, (double)n_rows * F * 4.0 * 2);
-    if (!reuse_softmax) {
-        stb::qk_softmax_kernel<<<stb::cdiv(n_rows, 8), 256, 0, st>>>(qk, n_rows, M, ldq, S, R, F, qk_scale, W, Fp);
-        STB_LAUNCH_OK();
-    }
-    stb::dyn_score_kernel<<<stb::cdiv(n_rows, 8), 256, 0, st>>>(W, n_rows, LH, R, F, Fp, prev_jumps, scores);
-    STB_LAUNCH_OK();
-    stb::dyn_select_kernel<<<dim3(R, B), 32, 0, st>>>(scores, LH, R, count, table);
-    STB_LAUNCH_OK();
-    stb::dyn_gather_kernel<<<dim3(R, count, B), 128, 0, st>>>(W, LH, R, Fp, count, table, Wsel);
-    STB_LAUNCH_OK();
-    stb::qk_znorm_kernel<<<dim3(stb::cdiv(F, 128), B * count), 128, 0, st>>>(Wsel, R, F, Fp);
-    STB_LAUNCH_OK();
-    stb::qk_median_mean_kernel<<<dim3(stb::cdiv(F, 128), R, B), 128, 0, st>>>(Wsel, count, R, F, Fp, medfilt_width, matrix, ldm);
-    STB_LAUNCH_OK();
-    return STB_OK;
+    if (!reuse_softmax)
+        STB_TRY(stb::launch(stb::qk_softmax_kernel, {stb::cdiv(n_rows, 8), 256, 0, st}, qk, n_rows, M, ldq, S, R, F, qk_scale, W, Fp));
+    STB_TRY(stb::launch(stb::dyn_score_kernel, {stb::cdiv(n_rows, 8), 256, 0, st}, W, n_rows, LH, R, F, Fp, prev_jumps, scores));
+    STB_TRY(stb::launch(stb::dyn_select_kernel, {dim3(R, B), 32, 0, st}, scores, LH, R, count, table));
+    STB_TRY(stb::launch(stb::dyn_gather_kernel, {dim3(R, count, B), 128, 0, st}, W, LH, R, Fp, count, table, Wsel));
+    STB_TRY(stb::launch(stb::qk_znorm_kernel, {dim3(stb::cdiv(F, 128), B * count), 128, 0, st}, Wsel, R, F, Fp));
+    return stb::launch(stb::qk_median_mean_kernel, {dim3(stb::cdiv(F, 128), R, B), 128, 0, st}, Wsel, count, R, F, Fp, medfilt_width,
+                       matrix, ldm);
 }
 
 extern "C" size_t stb_qkpost_new_ws_bytes(int B, int LH, int M, int F, int topk) {
@@ -408,15 +398,12 @@ extern "C" int stb_qk_postprocess_new(const float* qk, int B, int LH, int M, lon
     int32_t* top = (int32_t*)(score + (size_t)B * LH);
     const long long n_rows = (long long)B * LH * M;
     stb::ProfScope ps("qk_postprocess_new", st, (double)n_rows * F * 4.0 * 2);
-    stb::new_median_softmax_kernel<<<stb::cdiv(n_rows, 8), 256, 0, st>>>(qk, n_rows, ldq, F, qk_scale, medfilt_width, W, Fp);
-    STB_LAUNCH_OK();
-    stb::new_colstats_kernel<<<dim3(stb::cdiv(F, 128), B * LH), 128, 0, st>>>(W, M, F, Fp, colnorm, cover);
-    STB_LAUNCH_OK();
-    stb::new_score_kernel<<<B * LH, 256, 0, st>>>(W, colnorm, cover, M, F, Fp, w_colnorm, w_rownorm, w_coverage, score);
-    STB_LAUNCH_OK();
-    stb::new_topk_kernel<<<B, 32, 0, st>>>(score, LH, topk, top);
-    STB_LAUNCH_OK();
-    stb::new_matrix_kernel<<<dim3(stb::cdiv(F, 128), R, B), 128, 0, st>>>(W, colnorm, top, LH, M, S, F, Fp, topk, matrix, ldm, R);
-    STB_LAUNCH_OK();
-    return STB_OK;
+    STB_TRY(stb::launch(stb::new_median_softmax_kernel, {stb::cdiv(n_rows, 8), 256, 0, st}, qk, n_rows, ldq, F, qk_scale, medfilt_width,
+                        W, Fp));
+    STB_TRY(stb::launch(stb::new_colstats_kernel, {dim3(stb::cdiv(F, 128), B * LH), 128, 0, st}, W, M, F, Fp, colnorm, cover));
+    STB_TRY(stb::launch(stb::new_score_kernel, {B * LH, 256, 0, st}, W, colnorm, cover, M, F, Fp, w_colnorm, w_rownorm, w_coverage,
+                        score));
+    STB_TRY(stb::launch(stb::new_topk_kernel, {B, 32, 0, st}, score, LH, topk, top));
+    return stb::launch(stb::new_matrix_kernel, {dim3(stb::cdiv(F, 128), R, B), 128, 0, st}, W, colnorm, top, LH, M, S, F, Fp, topk,
+                       matrix, ldm, R);
 }

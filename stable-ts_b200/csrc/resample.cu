@@ -61,12 +61,8 @@ extern "C" int stb_resample_mono(const void* pcm, int sample_format, int channel
     long long blocks = (n_out + 255) / 256;
     const long long cap = (long long)stb::sm_count() * 16;
     if (blocks > cap) blocks = cap;
-    if (sample_format == 0)
-        stb::resample_mono_kernel<0><<<(unsigned)blocks, 256, 0, st>>>(pcm, channels, n_frames_in, L, M, table, taps, out, n_out, quantize_s16);
-    else if (sample_format == 1)
-        stb::resample_mono_kernel<1><<<(unsigned)blocks, 256, 0, st>>>(pcm, channels, n_frames_in, L, M, table, taps, out, n_out, quantize_s16);
-    else
-        stb::resample_mono_kernel<2><<<(unsigned)blocks, 256, 0, st>>>(pcm, channels, n_frames_in, L, M, table, taps, out, n_out, quantize_s16);
-    STB_LAUNCH_OK();
-    return STB_OK;
+    const auto kernel = sample_format == 0 ? stb::resample_mono_kernel<0>
+                        : sample_format == 1 ? stb::resample_mono_kernel<1>
+                                             : stb::resample_mono_kernel<2>;
+    return stb::launch(kernel, {(unsigned)blocks, 256, 0, st}, pcm, channels, n_frames_in, L, M, table, taps, out, n_out, quantize_s16);
 }

@@ -146,8 +146,6 @@ extern "C" int stb_silence_mask(const float* audio, int B, int n_samples, long l
     STB_REQUIRE(k_size == 0 || (k_size % 2 == 1 && k_size <= 31), "stb_silence_mask: kernel size must be odd");
     cudaStream_t st = (cudaStream_t)stream;
     stb::ProfScope ps("silence_mask", st, (double)B * n_samples * 4.0);
-    stb::silence_mask_kernel<<<B, stb::SIL_THREADS, 0, st>>>(audio, stride, n_samples, k, token_count, q_levels, k_size, thr_in,
-                                                            loudness_out, mask_out, thr_out);
-    STB_LAUNCH_OK();
-    return STB_OK;
+    return stb::launch(stb::silence_mask_kernel, {B, stb::SIL_THREADS, 0, st}, audio, stride, n_samples, k, token_count, q_levels,
+                       k_size, thr_in, loudness_out, mask_out, thr_out);
 }
