@@ -2,17 +2,26 @@
 // nothing but q, k, v^T and the output touches HBM.
 //
 // Replaces MultiHeadAttention.qkv_attention of whisper.model for the encoder's 1500 x 1500 self-attention
-// (reached from stable_whisper/timing.py:60 / decode.py:29).
+// (reached from stable_whisper/timing.py:60 / decode.py:29) and for the teacher-forced decoder's cross-attention in the
+// layers that a head list does not capture (engine.cu).
 //
 // One CTA = one (batch, head, 128-query tile); 9 warps:
 //   warps 0..3, 4..7  two consumer warpgroups of 64 query rows each: wgmma for both products, softmax in between
-//   warp 8            TMA producer: Q tile once, K tiles through a 2-stage ring (twice: pass 1 and pass 2), V^T tiles (pass 2)
+//   warp 8            TMA producer: Q tile once, then every 64-key K tile and V^T tile once, through a 4-stage K ring and
+//                     a 4-stage V^T ring that advance together
+// Registers bound the key tile: a consumer thread holds S_t, P_{t-1} (hi and lo), O and the Q fragments at once.  Under
+// __launch_bounds__(288, 1) ptxas gives this kernel at most 168 registers per thread (65536 / 384, as if the producer warp
+// were a whole warpgroup); so did a 384-thread variant whose producer warpgroup handed registers over by setmaxnreg.  At
+// that limit 128-key tiles use 168 registers, spill 240 bytes and serialise the wgmma; 64-key tiles take 154 registers
+// (122 with PASSES = 1) and do not spill.
 //
-// Exact two-pass softmax (same formula as the reference: exp(s - max) / sum), no accumulator rescaling:
-//   pass 1   S_t = Q K_t^T  (wgmma m64n128k16, operands in swizzled shared memory)  ->  row max m
-//   pass 2   S_t again      ->  p = exp(s - m)  ->  split fp16 (hi, lo): the accumulator fragment of 16 keys IS the A
-//            fragment of the next product, so P never leaves the registers  ->  O += P_t V_t  (wgmma m64n64k16, A from
-//            registers, V^T from shared memory), row sum l applied to O in the epilogue
+// One pass with an online softmax, in base-2 units (the 1/8 log2(e) scale folded into the exponent):
+//   S_t = Q K_t^T  (wgmma m64n64k16, Q from registers, K from swizzled shared memory)
+//   m' = max(m, rowmax S_t);  p = exp2(s - m');  l = l exp2(m - m') + rowsum p;  O = O exp2(m - m') + P_t V_t
+//   P_t is split fp16 (hi, lo): the accumulator fragment of 16 keys IS the A fragment of the next product, so P never leaves
+//   the registers (wgmma m64n64k16, A from registers, V^T from shared memory); O / l in the epilogue.
+// Overlap: a warpgroup issues S_t = Q K_t^T and O += P_{t-1} V_{t-1} together and computes the softmax of S_t while P.V
+// still runs; the two warpgroups take turns to issue (named barriers), so one's softmax runs under the other's MMAs.
 // Split precision as in the GEMM core: every product is hi*hi + hi*lo + lo*hi (3 MMA passes), fp32 accumulation.
 #include "common.cuh"
 #include "kernels.h"
@@ -20,7 +29,8 @@
 namespace stb {
 
 constexpr int AT_BQ = 128;       // queries per CTA
-constexpr int AT_BK = 128;       // keys per tile
+constexpr int AT_BK = 64;        // keys per tile
+constexpr int AT_STAGES = 4;     // K and V^T ring depth
 constexpr int AT_THREADS = 288;
 
 struct AttnArgs {
@@ -35,12 +45,12 @@ template <int PASSES>
 struct AttnCfg {
     static constexpr int NPL = PASSES == 3 ? 2 : 1;
     static constexpr uint32_t Q_TILE = AT_BQ * 128;                 // 16 KB: 128 rows x 128 B
-    static constexpr uint32_t K_TILE = AT_BK * 128;                 // 16 KB
-    static constexpr uint32_t V_CHUNK = 64 * 128;                   // 8 KB: 64 head dims x 64 keys
+    static constexpr uint32_t K_TILE = AT_BK * 128;                 // 8 KB: 64 keys x 64 head dims
+    static constexpr uint32_t V_TILE = 64 * AT_BK * 2;              // 8 KB: 64 head dims x 64 keys
     static constexpr uint32_t OFF_Q = 0;
-    static constexpr uint32_t OFF_K = OFF_Q + NPL * Q_TILE;         // 2 stages x NPL x K_TILE
-    static constexpr uint32_t OFF_V = OFF_K + 2 * NPL * K_TILE;     // 2 stages x NPL x 2 chunks
-    static constexpr uint32_t SMEM = OFF_V + 2 * NPL * 2 * V_CHUNK + 1024;
+    static constexpr uint32_t OFF_K = OFF_Q + NPL * Q_TILE;         // stages x NPL x K_TILE
+    static constexpr uint32_t OFF_V = OFF_K + AT_STAGES * NPL * K_TILE;
+    static constexpr uint32_t SMEM = OFF_V + AT_STAGES * NPL * V_TILE + 1024;
 };
 
 __device__ __forceinline__ void pick3(const int (&perm)[3], int row, int h, int b, int& c1, int& c2, int& c3) {
@@ -54,6 +64,19 @@ __device__ __forceinline__ uint32_t pack_h2(__half a, __half b) {
     return (uint32_t)__half_as_ushort(a) | ((uint32_t)__half_as_ushort(b) << 16);
 }
 
+// named barriers 1 and 2 (0 is __syncthreads) between the two consumer warpgroups
+template <int ID>
+__device__ __forceinline__ void named_bar_sync() { asm volatile("bar.sync %0, 256;" ::"n"(ID) : "memory"); }
+template <int ID>
+__device__ __forceinline__ void named_bar_arrive() { asm volatile("bar.arrive %0, 256;" ::"n"(ID) : "memory"); }
+
+// keeps the compiler from moving reads or writes of a wgmma accumulator across the wgmma_wait that makes it valid
+template <int N>
+__device__ __forceinline__ void fence_regs(float (&r)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
+}
+
 template <int PASSES>
 __global__ void __launch_bounds__(AT_THREADS, 1)
 attention_tc_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUtensorMap tmQl,
@@ -63,7 +86,7 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_const
     constexpr int NPL = Cfg::NPL;
     extern __shared__ uint8_t smem_dyn[];
     uint8_t* sm = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
-    __shared__ __align__(8) uint64_t q_full, k_full[2], k_empty[2], v_full[2], v_empty[2];
+    __shared__ __align__(8) uint64_t q_full, k_full[AT_STAGES], k_empty[AT_STAGES], v_full[AT_STAGES], v_empty[AT_STAGES];
 
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
     const int lane = threadIdx.x & 31;
@@ -75,7 +98,7 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_const
         tma_prefetch_desc(&tmQh); tma_prefetch_desc(&tmKh); tma_prefetch_desc(&tmVh);
         if (NPL == 2) { tma_prefetch_desc(&tmQl); tma_prefetch_desc(&tmKl); tma_prefetch_desc(&tmVl); }
         mbar_init(&q_full, 1);
-        for (int i = 0; i < 2; ++i) {                            // "empty": one arrival per consumer warpgroup
+        for (int i = 0; i < AT_STAGES; ++i) {                    // "empty": one arrival per consumer warpgroup
             mbar_init(&k_full[i], 1); mbar_init(&k_empty[i], 2);
             mbar_init(&v_full[i], 1); mbar_init(&v_empty[i], 2);
         }
@@ -91,29 +114,21 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_const
             mbar_arrive_expect_tx(&q_full, NPL * Cfg::Q_TILE);
             tma_load_4d(sm + Cfg::OFF_Q, &tmQh, &q_full, 0, c1, c2, c3);
             if (NPL == 2) tma_load_4d(sm + Cfg::OFF_Q + Cfg::Q_TILE, &tmQl, &q_full, 0, c1, c2, c3);
-            for (int i = 0; i < 2 * NT; ++i) {
-                const int t = i % NT, st = i & 1;
-                const uint32_t ph = (i >> 1) & 1;
+            for (int t = 0; t < NT; ++t) {
+                const int st = t % AT_STAGES;
+                const uint32_t ph = (t / AT_STAGES) & 1;
                 mbar_wait_mma(&k_empty[st], ph ^ 1);
                 mbar_arrive_expect_tx(&k_full[st], NPL * Cfg::K_TILE);
                 pick3(g.permK, t * AT_BK, h, b, c1, c2, c3);
                 uint8_t* kd = sm + Cfg::OFF_K + st * NPL * Cfg::K_TILE;
                 tma_load_4d(kd, &tmKh, &k_full[st], 0, c1, c2, c3);
                 if (NPL == 2) tma_load_4d(kd + Cfg::K_TILE, &tmKl, &k_full[st], 0, c1, c2, c3);
-                if (i >= NT) {                                   // pass 2: the V^T tile of the same keys
-                    const int vs = t & 1;
-                    const uint32_t vph = (t >> 1) & 1;
-                    mbar_wait_mma(&v_empty[vs], vph ^ 1);
-                    mbar_arrive_expect_tx(&v_full[vs], NPL * 2 * Cfg::V_CHUNK);
-                    pick3(g.permV, 0, h, b, c1, c2, c3);
-                    uint8_t* vd = sm + Cfg::OFF_V + vs * NPL * 2 * Cfg::V_CHUNK;
-                    tma_load_4d(vd, &tmVh, &v_full[vs], t * AT_BK, c1, c2, c3);
-                    tma_load_4d(vd + Cfg::V_CHUNK, &tmVh, &v_full[vs], t * AT_BK + 64, c1, c2, c3);
-                    if (NPL == 2) {
-                        tma_load_4d(vd + 2 * Cfg::V_CHUNK, &tmVl, &v_full[vs], t * AT_BK, c1, c2, c3);
-                        tma_load_4d(vd + 3 * Cfg::V_CHUNK, &tmVl, &v_full[vs], t * AT_BK + 64, c1, c2, c3);
-                    }
-                }
+                mbar_wait_mma(&v_empty[st], ph ^ 1);                 // the V^T tile of the same keys
+                mbar_arrive_expect_tx(&v_full[st], NPL * Cfg::V_TILE);
+                pick3(g.permV, 0, h, b, c1, c2, c3);
+                uint8_t* vd = sm + Cfg::OFF_V + st * NPL * Cfg::V_TILE;
+                tma_load_4d(vd, &tmVh, &v_full[st], t * AT_BK, c1, c2, c3);
+                if (NPL == 2) tma_load_4d(vd + Cfg::V_TILE, &tmVl, &v_full[st], t * AT_BK, c1, c2, c3);
             }
         }
         return;
@@ -124,108 +139,164 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_const
     const bool leader = (threadIdx.x & 127) == 0;
     const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // fragment row r inside the CTA's query tile
     const int colq = 2 * (lane & 3);
-    const uint32_t q_hi = smem_u32(sm + Cfg::OFF_Q) + (uint32_t)wg * 64u * 128u, q_lo = q_hi + Cfg::Q_TILE;
     constexpr float LOG2E = 1.4426950408889634f;
     const float sc = 0.125f * LOG2E;                           // scores in log2 units: exp(x) = exp2(x * log2e)
-    mbar_wait_mma(&q_full, 0);
 
-    float s[64];
-    // S = Q K_t^T for K ring use i (64 x 128 per warpgroup), then the K slot is released
-    auto scores = [&](int i) {
-        const int st = i & 1;
-        mbar_wait_mma(&k_full[st], (i >> 1) & 1);
-        const uint32_t k_hi = smem_u32(sm + Cfg::OFF_K + st * NPL * Cfg::K_TILE), k_lo = k_hi + Cfg::K_TILE;
-        uint32_t accum = 0;
+    // Issue turns alternate between the warpgroups, warpgroup 0 first: a warpgroup waits on its own barrier before it
+    // issues and arrives on the other's after.  Both make NT + 1 turns; warpgroup 1's initial arrival stands in for its
+    // last one, so every barrier phase is completed.
+    if (wg == 1) named_bar_arrive<1>();
+    int turn = 0;
+    auto turn_begin = [&] {
+        if (wg == 0) named_bar_sync<1>(); else named_bar_sync<2>();
         wgmma_fence();
-#pragma unroll
-        for (int pass = 0; pass < PASSES; ++pass) {
-            const uint32_t pa = (pass == 2) ? q_lo : q_hi;
-            const uint32_t pb = (pass == 1) ? k_lo : k_hi;
-#pragma unroll
-            for (int k4 = 0; k4 < 4; ++k4) {
-                wgmma_ss(s, wgmma_desc_k128(pa + k4 * 32), wgmma_desc_k128(pb + k4 * 32), accum);
-                accum = 1;
-            }
-        }
-        wgmma_commit();
-        wgmma_wait<0>();
-        if (leader) mbar_arrive(&k_empty[st]);
+    };
+    auto turn_end = [&] {
+        if (wg == 0) named_bar_arrive<2>(); else if (++turn <= NT) named_bar_arrive<1>();
     };
 
-    // ---------------- pass 1: row max only (the sum is accumulated in pass 2 and applied to O in the epilogue:
-    // softmax(s) v == (sum_j exp(s_j - m) v_j) / (sum_j exp(s_j - m)))
-    float m0 = -INFINITY, m1 = -INFINITY;
-    for (int t = 0; t < NT; ++t) {
-        scores(t);
-        const int kbase = t * AT_BK + colq;
-        const bool full_tile = (t + 1) * AT_BK <= g.Mk;        // warp-uniform: no per-element key masking needed
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-                if (full_tile || kbase + 8 * j + e < g.Mk) {
-                    m0 = fmaxf(m0, s[4 * j + e]);
-                    m1 = fmaxf(m1, s[4 * j + 2 + e]);
-                }
-            }
-        }
-    }
-    m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 1));
-    m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 2)) * sc;  // row max in log2 units
-    m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 1));
-    m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 2)) * sc;
-
-    // ---------------- pass 2: S again -> p = exp(s - m) -> split fp16 (hi, lo) A fragments in registers -> O += P_t V_t
+    float s[32];                                               // S_t, then exp2(s - m) in place
     float o[32];
 #pragma unroll
     for (int i = 0; i < 32; ++i) o[i] = 0.f;
-    float l0 = 0.f, l1 = 0.f;
-    uint32_t o_accum = 0;
-    for (int t = 0; t < NT; ++t) {
-        scores(NT + t);
-        const int kbase = t * AT_BK + colq;
-        const bool full_tile = (t + 1) * AT_BK <= g.Mk;
-        // the score fragment of 16 keys (two 8-column groups) is exactly the m64k16 A fragment of the same rows
-        uint32_t p_hi[8][4], p_lo[8][4];
+    uint32_t p_hi[4][4], p_lo[4][4];                           // P_{t-1}: the A fragments of the P.V product in flight
+    float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+
+    mbar_wait_mma(&q_full, 0);
+    // Q as m64k16 A fragments in registers (loaded once from the swizzled tile), so that Q K^T reads only K from shared
+    // memory: with both operands there, a 64-key product would need all of the SM's shared-memory bandwidth
+    uint32_t qa[NPL][4][4];
 #pragma unroll
-        for (int kc = 0; kc < 8; ++kc) {
+    for (int pl = 0; pl < NPL; ++pl)
+#pragma unroll
+        for (int k4 = 0; k4 < 4; ++k4)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {                        // i = 2 (k + 8 ?) + (row r + 8 ?)
+                const int rr = row + 8 * (i & 1), cb = 2 * (16 * k4 + 8 * (i >> 1) + colq);   // byte column in the row
+                qa[pl][k4][i] = *reinterpret_cast<const uint32_t*>(sm + Cfg::OFF_Q + pl * Cfg::Q_TILE + rr * 128 +
+                                                                    ((((cb >> 4) ^ (rr & 7))) << 4) + (cb & 15));
+            }
+    auto issue_scores = [&](int t) {                           // S = Q K_t^T (64 x 64 per warpgroup)
+        const uint32_t k_hi = smem_u32(sm + Cfg::OFF_K + (t % AT_STAGES) * NPL * Cfg::K_TILE), k_lo = k_hi + Cfg::K_TILE;
+#pragma unroll
+        for (int pass = 0; pass < PASSES; ++pass) {
+            const uint32_t pb = (pass == 1) ? k_lo : k_hi;
+#pragma unroll
+            for (int k4 = 0; k4 < 4; ++k4)
+                wgmma_rs(s, qa[pass == 2 ? NPL - 1 : 0][k4], wgmma_desc_k128(pb + k4 * 32), pass + k4 > 0);
+        }
+        wgmma_commit();
+    };
+    auto issue_pv = [&](int t) {                               // O += P_t V_t
+        const uint32_t v_base = smem_u32(sm + Cfg::OFF_V + (t % AT_STAGES) * NPL * Cfg::V_TILE);
+#pragma unroll
+        for (int pass = 0; pass < PASSES; ++pass) {
+            const uint32_t pb = v_base + ((pass == 1) ? Cfg::V_TILE : 0);
+#pragma unroll
+            for (int kc = 0; kc < 4; ++kc) {                     // 64 keys = 4 k-steps of 16
+                const uint64_t vd = wgmma_desc_k128(pb + kc * 32);
+                if (pass == 2) wgmma_rs(o, p_lo[kc], vd, 1); else wgmma_rs(o, p_hi[kc], vd, 1);
+            }
+        }
+        wgmma_commit();
+    };
+    // the new row maxima from S_t, p = exp2(s - m) in place, l rescaled and summed; returns the O rescale factors
+    auto softmax = [&](int t, float& a0, float& a1) {
+        fence_regs(s);
+        if ((t + 1) * AT_BK > g.Mk) {                          // the partial last tile: keys past Mk do not exist
+            const int kbase = t * AT_BK + colq;
+#pragma unroll
+            for (int j = 0; j < 8; ++j)
+#pragma unroll
+                for (int e = 0; e < 2; ++e)
+                    if (kbase + 8 * j + e >= g.Mk) s[4 * j + e] = s[4 * j + 2 + e] = -INFINITY;
+        }
+        float x0 = -INFINITY, x1 = -INFINITY;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            x0 = fmaxf(x0, fmaxf(s[4 * j], s[4 * j + 1]));
+            x1 = fmaxf(x1, fmaxf(s[4 * j + 2], s[4 * j + 3]));
+        }
+        x0 = fmaxf(x0, __shfl_xor_sync(0xffffffffu, x0, 1));
+        x0 = fmaxf(x0, __shfl_xor_sync(0xffffffffu, x0, 2));
+        x1 = fmaxf(x1, __shfl_xor_sync(0xffffffffu, x1, 1));
+        x1 = fmaxf(x1, __shfl_xor_sync(0xffffffffu, x1, 2));
+        const float n0 = fmaxf(m0, x0 * sc), n1 = fmaxf(m1, x1 * sc);   // finite: every tile has a key
+        a0 = exp2f(m0 - n0);                                   // 0 on the first tile (m = -inf)
+        a1 = exp2f(m1 - n1);
+        m0 = n0;
+        m1 = n1;
+        float r0 = 0.f, r1 = 0.f;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                s[4 * j + e] = exp2f(fmaf(s[4 * j + e], sc, -n0));
+                s[4 * j + 2 + e] = exp2f(fmaf(s[4 * j + 2 + e], sc, -n1));
+                r0 += s[4 * j + e];
+                r1 += s[4 * j + 2 + e];
+            }
+        }
+        l0 = fmaf(l0, a0, r0);
+        l1 = fmaf(l1, a1, r1);
+    };
+    // P_t = split fp16 of s: the score fragment of 16 keys (two 8-column groups) is exactly the m64k16 A fragment
+    auto split_p = [&] {
+#pragma unroll
+        for (int kc = 0; kc < 4; ++kc) {
 #pragma unroll
             for (int q = 0; q < 4; ++q) {                        // q = 2 (column group within the chunk) + (row r + 8 ?)
-                const int j = 2 * kc + (q >> 1);
-                float pv[2];
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                    const float mrow = (q & 1) ? m1 : m0;
-                    float pe = exp2f(fmaf(s[4 * j + 2 * (q & 1) + e], sc, -mrow));
-                    if (!full_tile && kbase + 8 * j + e >= g.Mk) pe = 0.f;
-                    pv[e] = pe;
-                }
-                if (q & 1) l1 += pv[0] + pv[1]; else l0 += pv[0] + pv[1];
+                const int i = 4 * (2 * kc + (q >> 1)) + 2 * (q & 1);
                 __half h0, lo0, h1, lo1;
-                split_f16(pv[0], h0, lo0);
-                split_f16(pv[1], h1, lo1);
+                split_f16(s[i], h0, lo0);
+                split_f16(s[i + 1], h1, lo1);
                 p_hi[kc][q] = pack_h2(h0, h1);
                 p_lo[kc][q] = pack_h2(lo0, lo1);
             }
         }
-        const int vs = t & 1;
-        mbar_wait_mma(&v_full[vs], (t >> 1) & 1);
-        const uint32_t v_base = smem_u32(sm + Cfg::OFF_V + vs * NPL * 2 * Cfg::V_CHUNK);
-        wgmma_fence();
+    };
+    auto rescale_o = [&](float a0, float a1) {
+        fence_regs(o);
 #pragma unroll
-        for (int pass = 0; pass < PASSES; ++pass) {
-            const uint32_t pb = v_base + ((pass == 1) ? 2 * Cfg::V_CHUNK : 0);
-#pragma unroll
-            for (int kc = 0; kc < 8; ++kc) {                     // 128 keys = 2 chunks x 4 k-steps of 16
-                const uint64_t vd = wgmma_desc_k128(pb + (kc >> 2) * Cfg::V_CHUNK + (kc & 3) * 32);
-                if (pass == 2) wgmma_rs(o, p_lo[kc], vd, o_accum); else wgmma_rs(o, p_hi[kc], vd, o_accum);
-                o_accum = 1;
-            }
+        for (int j = 0; j < 8; ++j) {
+            o[4 * j] *= a0; o[4 * j + 1] *= a0;
+            o[4 * j + 2] *= a1; o[4 * j + 3] *= a1;
         }
-        wgmma_commit();
+    };
+
+    float a0, a1;
+    auto full = [&](uint64_t* bars, int t) { mbar_wait_mma(&bars[t % AT_STAGES], (t / AT_STAGES) & 1); };
+    auto release = [&](uint64_t* bars, int t) { if (leader) mbar_arrive(&bars[t % AT_STAGES]); };
+    full(k_full, 0);
+    turn_begin();
+    issue_scores(0);
+    turn_end();
+    wgmma_wait<0>();
+    release(k_empty, 0);
+    softmax(0, a0, a1);                                        // O is still zero: no rescale
+    split_p();
+    for (int t = 1; t < NT; ++t) {
+        full(k_full, t);
+        full(v_full, t - 1);
+        turn_begin();
+        issue_scores(t);
+        issue_pv(t - 1);
+        turn_end();
+        wgmma_wait<1>();                                       // S_t is ready; P_{t-1} V_{t-1} may still run
+        release(k_empty, t);
+        softmax(t, a0, a1);
         wgmma_wait<0>();
-        if (leader) mbar_arrive(&v_empty[vs]);
+        release(v_empty, t - 1);
+        rescale_o(a0, a1);
+        split_p();
     }
+    full(v_full, NT - 1);
+    turn_begin();
+    issue_pv(NT - 1);
+    turn_end();
+    wgmma_wait<0>();
+    fence_regs(o);
+
     // ---------------- epilogue: O / l -> split fp16 -> attention output
     l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
     l0 += __shfl_xor_sync(0xffffffffu, l0, 2);

@@ -316,11 +316,19 @@ static int decoder_forward(stb_model* m, const int32_t* tokens, int B, int M, co
         STB_TRY(layernorm(w.x, rows, d, W_F32(L, STB_L_CROSS_LN_G), W_F32(L, STB_L_CROSS_LN_B), w.ln.hi, w.ln.lo, nullptr, st));
         STB_TRY(linear(m, w.ln, rows, d, W_HI(L, STB_L_CQ_W), W_LO(L, STB_L_CQ_W), d,
                        ep_split(w.q, d, W_F32(L, STB_L_CQ_B), STB_ACT_NONE), st));
-        {
-            Split Kx, vTx;
-            cross_ptrs(m, B, ckv, l, Kx, vTx);
-            stb_operand q = opnd(w.q.hi, w.q.lo, M, 64, d, 64, (long long)M * d);
-            stb_operand k = opnd(Kx.hi, Kx.lo, T, 64, 64, (long long)T * 64, (long long)H * T * 64);   // head-major K
+        Split Kx, vTx;
+        cross_ptrs(m, B, ckv, l, Kx, vTx);
+        stb_operand q = opnd(w.q.hi, w.q.lo, M, 64, d, 64, (long long)M * d);
+        stb_operand k = opnd(Kx.hi, Kx.lo, T, 64, 64, (long long)T * 64, (long long)H * T * 64);   // head-major K
+        stb_operand v = opnd(vTx.hi, vTx.lo, 64, Tp, Tp, 64LL * Tp, (long long)d * Tp);
+        // A layer none of whose heads is in a given head list runs the fused kernel, which keeps the scores in registers.
+        // A pass that captures nothing keeps the unfused route: its logits match those of the same pass with every head
+        // captured (the model-object protocol with and without forward hooks) to the last bits.
+        bool fused = qk_out != nullptr && n_sel >= 0;
+        for (int i = 0; fused && i < n_sel; ++i) fused = sel[2 * i] != l;
+        if (fused) {
+            STB_TRY(fused_attention(q, k, v, B, H, M, T, w.attn.hi, w.attn.lo, d, 64, (long long)M * d, st));
+        } else {
             stb_epilogue e = ep_f32(w.Sx, Tp, nullptr, nullptr, 0, 0.125f);
             e.out_h_stride = (long long)M * Tp;
             e.out_b_stride = (long long)H * M * Tp;
@@ -346,7 +354,6 @@ static int decoder_forward(stb_model* m, const int32_t* tokens, int B, int M, co
             }
             STB_TRY(softmax_rows(w.Sx, (long long)B * H * M, T, Tp, M, 0, w.Px.hi, w.Px.lo, Tp, st));
             stb_operand p = opnd(w.Px.hi, w.Px.lo, M, Tp, Tp, (long long)M * Tp, (long long)H * M * Tp);
-            stb_operand v = opnd(vTx.hi, vTx.lo, 64, Tp, Tp, 64LL * Tp, (long long)d * Tp);
             stb_epilogue eo = ep_split(w.attn, d, nullptr, STB_ACT_NONE, 64, (long long)M * d);
             STB_TRY(gemm(p, v, B, H, eo, st));
         }

@@ -4,7 +4,9 @@ rotating weight copies exceeds the 126 MB L2 so every launch streams its weights
     python tools/microbench.py gemv      # decode-step linear shapes of large-v3 at 16 / 64 sequences
     python tools/microbench.py dtw       # DTW at 16 / 64 windows x [101 x 1500]
     python tools/microbench.py step 120 4   # ms per decode step (120 windows, 4 decoder layers of large-v3 width)
+    python tools/microbench.py attention # encoder attention (stb_attention) at 48 windows x 20 heads x 1500 x 1500
 """
+import ctypes
 import json
 import os
 import sys
@@ -85,6 +87,59 @@ def bench_dtw(batches=(16, 64, 148)):
     return out
 
 
+def _card():
+    """name, power limit and max SM clock of the current device, read next to the measurement they qualify"""
+    import subprocess
+    p = torch.cuda.get_device_properties(torch.cuda.current_device())
+    # nvidia-smi numbers the cards in PCI order, whatever CUDA_VISIBLE_DEVICES makes of them: select by PCI address
+    pci = f"{p.pci_domain_id:08X}:{p.pci_bus_id:02X}:{p.pci_device_id:02X}.0"
+    info = {"name": p.name, "pci_bus_id": pci}
+    try:
+        q = subprocess.run(["nvidia-smi", f"--id={pci}", "--query-gpu=power.limit,clocks.max.sm",
+                            "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=30).stdout.strip()
+        pl, mhz = (v.strip() for v in q.split(","))
+        info.update(power_limit_w=float(pl), sm_max_mhz=int(mhz))
+    except Exception as e:
+        info["nvidia_smi"] = f"unavailable: {e}"
+    return info
+
+
+def bench_attention(windows=48, heads=20, T=1500, iters=10):
+    """stb_attention at the encoder's shape (large-v3: 20 heads of 64, 1500 x 1500, one launch per layer for all windows).
+    Algorithmic work is 4 T^2 64 per (window, head); executed work counts the fp16 passes of every product (3 in parity
+    mode, 1 in fp16 mode).  The peak is the H100 SXM data sheet's dense fp16 rate, not a measured one."""
+    lib = L.lib()
+    d, ldk = 64 * heads, (T + 7) // 8 * 8
+    g = torch.Generator(device="cuda").manual_seed(0)
+    x = torch.randn(windows, T, 2 * d, device="cuda", generator=g)           # q | k, as the encoder's fused projection
+    vT = torch.zeros(windows, heads, 64, ldk, device="cuda")
+    vT[..., :T] = torch.randn(windows, heads, 64, T, device="cuda", generator=g)
+    xh, vh = x.half(), vT.half()
+    xl, vl = (x - xh.float()).half(), (vT - vh.float()).half()
+    del x, vT
+    out_hi = torch.empty(windows, T, d, dtype=torch.float16, device="cuda")
+    out_lo = torch.empty_like(out_hi)
+    flop = 4.0 * T * T * 64 * heads * windows
+    res = {"card": _card(), "shape": dict(windows=windows, heads=heads, Mq=T, Mk=T), "algorithmic_gflop_per_launch": flop / 1e9,
+           "peak_tflops": 989.0, "peak_source": "H100 SXM data sheet, dense fp16 at 700 W (not measured)", "runs": []}
+    for passes in (3, 1):
+        lo = passes == 3
+        oq = L.Operand(L.ptr(xh), L.ptr(xl) if lo else None, T, 64, 2 * d, 64, T * 2 * d)
+        ok = L.Operand(L.ptr(xh[..., d:]), L.ptr(xl[..., d:]) if lo else None, T, 64, 2 * d, 64, T * 2 * d)
+        ov = L.Operand(L.ptr(vh), L.ptr(vl) if lo else None, 64, ldk, ldk, 64 * ldk, d * ldk)
+
+        def run(i):
+            L.check(lib.stb_attention(ctypes.byref(oq), ctypes.byref(ok), ctypes.byref(ov), windows, heads, T, T,
+                                      L.ptr(out_hi), L.ptr(out_lo) if lo else None, d, 64, T * d, L.stream_ptr()))
+        us = _time(run, iters)
+        alg = flop / (us * 1e-6) / 1e12
+        res["runs"].append(dict(passes=passes, us_per_launch=round(us, 1), algorithmic_tflops=round(alg, 1),
+                                executed_tflops=round(alg * passes, 1), executed_frac_of_peak=round(alg * passes / 989.0, 3)))
+        print(res["runs"][-1], flush=True)
+    print(res["card"], flush=True)
+    return res
+
+
 def bench_step(windows=120, layers=4, s1=24, s2=72):
     """ms per KV-cached decode step of a large-v3-WIDTH model with `layers` decoder layers (cross K/V of 120 windows x 32
     layers would not leave room for A/B runs), from the slope between two forced decodes of s1 and s2 steps (graph replay):
@@ -133,5 +188,5 @@ if __name__ == "__main__":
     elif what == "ncu":          # short run for `ncu -k regex:...`: fc1 / fc2 at 64 sequences + one DTW batch
         res = [bench_gemv((64,), ((5120, 1280), (1280, 5120)), iters=4), bench_dtw((16,))]
     else:
-        res = {"gemv": bench_gemv, "dtw": bench_dtw}[what]()
+        res = {"gemv": bench_gemv, "dtw": bench_dtw, "attention": bench_attention}[what]()
     print(json.dumps({what: res, "env": {k: v for k, v in os.environ.items() if k.startswith("STB_")}}))
