@@ -101,9 +101,10 @@ typedef struct {
 
 STB_API int stb_gemm(const stb_operand* A, const stb_operand* B, int n_batch, int n_head, const stb_epilogue* ep, void* stream);
 
-/* Fused attention (K4): out[b][m][h*64 + c] = softmax(q k^T / 8) v with scores kept in registers (wgmma) and the
- * probabilities passed through shared memory.  q: rows Mq, k = 64; k: rows Mk, k = 64; vT: rows 64, k >= Mk (zero padded
- * keys).  Output split planes with offsets b*out_b_stride + h*out_h_stride + m*ld_out + c.  Non-causal (encoder). */
+/* Fused attention (K4): out[b][m][h*64 + c] = softmax(q k^T / 8) v with the scores and probabilities kept in registers
+ * (wgmma, one pass over the keys with an online softmax).  q: rows Mq, k = 64; k: rows Mk, k = 64; vT: rows 64, k >= Mk
+ * (zero padded keys).  Output split planes with offsets b*out_b_stride + h*out_h_stride + m*ld_out + c.  Non-causal: the
+ * encoder's self-attention and the teacher-forced decoder's cross-attention. */
 STB_API int stb_attention(const stb_operand* q, const stb_operand* k, const stb_operand* vT, int n_batch, int n_head, int Mq,
                   int Mk, void* out_hi, void* out_lo, long long ld_out, long long out_h_stride, long long out_b_stride,
                   void* stream);
@@ -187,7 +188,9 @@ STB_API int stb_cross_kv(stb_model* m, const void* xa_hi, const void* xa_lo, int
 /* a3 teacher-forced decoder with cross-attention capture (stable_whisper/timing.py:50-61 under disable_sdpa).
  *   tokens [B][M] int32.  logits (nullable) [B*M][ld_logits] fp32.
  *   qk_out (nullable) fp32 [B][n_sel][M][STB_KPAD]: scaled PRE-softmax cross-attention scores of the selected
- *   (layer, head) pairs sel_pairs_host[2*n_sel] (host array); n_sel < 0 selects all L*H heads in (layer, head) order. */
+ *   (layer, head) pairs sel_pairs_host[2*n_sel] (host array); n_sel < 0 selects all L*H heads in (layer, head) order.
+ *   Columns 1500..STB_KPAD-1 of each qk_out row are not written.
+ *   The logits do not depend on qk_out, sel_pairs_host or n_sel: a pass computes them the same way whatever it captures. */
 STB_API size_t stb_decoder_ws_bytes(const stb_model* m, int B, int M);
 STB_API int stb_decoder_forward(stb_model* m, const int32_t* tokens, int B, int M, const void* cross_kv, float* logits,
                         long long ld_logits, float* qk_out, const int32_t* sel_pairs_host, int n_sel, void* ws,

@@ -2,8 +2,8 @@
 // nothing but q, k, v^T and the output touches HBM.
 //
 // Replaces MultiHeadAttention.qkv_attention of whisper.model for the encoder's 1500 x 1500 self-attention
-// (reached from stable_whisper/timing.py:60 / decode.py:29) and for the teacher-forced decoder's cross-attention in the
-// layers that a head list does not capture (engine.cu).
+// (reached from stable_whisper/timing.py:60 / decode.py:29) and for the teacher-forced decoder's cross-attention
+// (engine.cu).  Scores a caller captures come from a GEMM of their own.
 //
 // One CTA = one (batch, head, 128-query tile); 9 warps:
 //   warps 0..3, 4..7  two consumer warpgroups of 64 query rows each: wgmma for both products, softmax in between

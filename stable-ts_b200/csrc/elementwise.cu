@@ -203,28 +203,6 @@ int zero_pad_rows(__half* hi, __half* lo, int B, int C, int T, cudaStream_t st) 
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// Cross-attention capture: copy the scaled pre-softmax scores of selected heads of one layer,
-// S [B][H][M][ld] -> qk_out [B][n_sel][M][ld] (what the forward hooks of stable_whisper/timing.py:51-56 collect).
-// ---------------------------------------------------------------------------------------------------------
-__global__ void capture_kernel(const float* __restrict__ S, int H, long long slice, float* __restrict__ out, int n_sel,
-                               CaptureList list) {
-    const int which = blockIdx.y, b = blockIdx.z;
-    const float4* src = reinterpret_cast<const float4*>(S + ((long long)b * H + list.head[which]) * slice);
-    float4* dst = reinterpret_cast<float4*>(out + ((long long)b * n_sel + list.slot[which]) * slice);
-    const long long n4 = slice >> 2;
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x)
-        dst[i] = src[i];
-}
-int capture_heads(const float* S, int B, int H, int M, long long ld, float* out, int n_sel, const CaptureList& list,
-                  cudaStream_t st) {
-    if (list.count == 0) return STB_OK;
-    const long long slice = (long long)M * ld;
-    STB_REQUIRE(slice % 4 == 0, "capture: slice not a multiple of 4 floats");
-    dim3 grid(min(cdiv(slice / 4, 256), 64), list.count, B);
-    return launch(capture_kernel, {grid, 256, 0, st}, S, H, slice, out, n_sel, list);
-}
-
-// ---------------------------------------------------------------------------------------------------------
 // Token probability (+ rank): p = softmax(logits[r][:n_classes])[target[r]]; rank = #classes with logit < target's.
 // One CTA per row (n_classes ~ 50k fp32 = 200 KB: a streaming read, two passes served by L2).
 // ---------------------------------------------------------------------------------------------------------

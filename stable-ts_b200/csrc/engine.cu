@@ -8,7 +8,8 @@
 // Data layout in HBM (all caller-owned):
 //   residual stream          fp32  [rows][d]
 //   GEMM inputs              split fp16 planes written by the producing kernel's epilogue (LayerNorm, GELU, softmax...)
-//   attention scores         fp32  [B][H][Mq][ldk]  (ldk = keys rounded up to 8); probabilities split, same shape
+//   self-attention scores    fp32  [B][H][Mq][ldk]  (decoder, causal; ldk = keys rounded up to 8); probabilities split,
+//                            same shape.  The encoder and the cross-attention keep them in registers (attention_tc.cu)
 //   V                        stored transposed [B][H][64][ldk] so P.V is a K-major GEMM
 //   conv inputs              time-major [B][T+2][C] with zero pad rows: overlapping TMA rows (stride C or 2C, width 3C)
 //                            are the im2col matrix, no copy
@@ -78,7 +79,7 @@ static stb_epilogue ep_f32(float* out, long long ld, const float* bias, const fl
 #define W_LO(layer, id) (m->prec == STB_PREC_FP16X3 ? (layer).p[id][1] : nullptr)
 #define W_F32(layer, id) ((const float*)(layer).p[id][0])
 
-// ---- one multi-head attention: scores, softmax, P.V.  q / k are split views with (row, head, batch) strides. ----
+// ---- one causal multi-head attention: scores, softmax, P.V.  q / k are split views with (row, head, batch) strides. ----
 struct AttnBufs {
     float* S;          // [B][H][Mq][ldk]
     Split P;           // same shape
@@ -87,13 +88,13 @@ struct AttnBufs {
 };
 
 static int attention(const stb_model* m, int B, int H, int d, int Mq, int Mk, int ldk, const stb_operand& q,
-                     const stb_operand& k, const AttnBufs& bufs, int causal, cudaStream_t st) {
+                     const stb_operand& k, const AttnBufs& bufs, cudaStream_t st) {
     // S = (q k^T) / 8  (whisper scales q and k by 64^-0.25 each; head_dim is 64 for every released model)
     stb_epilogue e = ep_f32(bufs.S, ldk, nullptr, nullptr, 0, 0.125f);
     e.out_h_stride = (long long)Mq * ldk;
     e.out_b_stride = (long long)H * Mq * ldk;
     STB_TRY(gemm(q, k, B, H, e, st));
-    STB_TRY(softmax_rows(bufs.S, (long long)B * H * Mq, Mk, ldk, Mq, causal, bufs.P.hi, bufs.P.lo, ldk, st));
+    STB_TRY(softmax_rows(bufs.S, (long long)B * H * Mq, Mk, ldk, Mq, 1, bufs.P.hi, bufs.P.lo, ldk, st));
     stb_operand p = opnd(bufs.P.hi, bufs.P.lo, Mq, ldk, ldk, (long long)Mq * ldk, (long long)H * Mq * ldk);
     stb_operand v = opnd(bufs.vT.hi, bufs.vT.lo, 64, ldk, ldk, 64LL * ldk, (long long)d * ldk);
     stb_epilogue eo = ep_split(bufs.out, d, nullptr, STB_ACT_NONE, 64, (long long)Mq * d);
@@ -260,15 +261,14 @@ static int cross_kv(stb_model* m, const __half* xa_hi, const __half* xa_lo, int 
 // ---------------------------------------------------------------------------------------------------------
 struct DecWs {
     float* x;
-    Split ln, qk, vT, Ps, attn, q, Px, hid;
+    Split ln, qk, vT, Ps, attn, q, hid;
     float* Ss;
-    float* Sx;
     size_t bytes;
 };
 static DecWs carve_decoder(const stb_model* m, int B, int M, void* ws) {
     const stb_dims& D = m->dims;
     const bool lo = m->prec == STB_PREC_FP16X3;
-    const size_t d = D.n_text_state, H = D.n_text_head, Tp = STB_KPAD, Mp = (M + 7) & ~7;
+    const size_t d = D.n_text_state, H = D.n_text_head, Mp = (M + 7) & ~7;
     Carver c(ws);
     DecWs w;
     w.x = c.take<float>((size_t)B * M * d);
@@ -279,8 +279,6 @@ static DecWs carve_decoder(const stb_model* m, int B, int M, void* ws) {
     w.Ps = take_split(c, (size_t)B * H * M * Mp, lo);
     w.attn = take_split(c, (size_t)B * M * d, lo);
     w.q = take_split(c, (size_t)B * M * d, lo);
-    w.Sx = c.take<float>((size_t)B * H * M * Tp);
-    w.Px = take_split(c, (size_t)B * H * M * Tp, lo);
     w.hid = take_split(c, (size_t)B * M * 4 * d, lo);
     w.bytes = c.off;
     return w;
@@ -308,7 +306,7 @@ static int decoder_forward(stb_model* m, const int32_t* tokens, int B, int M, co
             stb_operand q = opnd(w.qk.hi, w.qk.lo, M, 64, 2 * d, 64, (long long)M * 2 * d);
             stb_operand k = opnd(offs(w.qk.hi, d), offs(w.qk.lo, d), M, 64, 2 * d, 64, (long long)M * 2 * d);
             AttnBufs ab = {w.Ss, w.Ps, w.vT, w.attn};
-            STB_TRY(attention(m, B, H, d, M, M, Mp, q, k, ab, 1, st));
+            STB_TRY(attention(m, B, H, d, M, M, Mp, q, k, ab, st));
         }
         STB_TRY(linear(m, w.attn, rows, d, W_HI(L, STB_L_OUT_W), W_LO(L, STB_L_OUT_W), d,
                        ep_f32(w.x, d, W_F32(L, STB_L_OUT_B), w.x, d), st));
@@ -321,41 +319,24 @@ static int decoder_forward(stb_model* m, const int32_t* tokens, int B, int M, co
         stb_operand q = opnd(w.q.hi, w.q.lo, M, 64, d, 64, (long long)M * d);
         stb_operand k = opnd(Kx.hi, Kx.lo, T, 64, 64, (long long)T * 64, (long long)H * T * 64);   // head-major K
         stb_operand v = opnd(vTx.hi, vTx.lo, 64, Tp, Tp, 64LL * Tp, (long long)d * Tp);
-        // A layer none of whose heads is in a given head list runs the fused kernel, which keeps the scores in registers.
-        // A pass that captures nothing keeps the unfused route: its logits match those of the same pass with every head
-        // captured (the model-object protocol with and without forward hooks) to the last bits.
-        bool fused = qk_out != nullptr && n_sel >= 0;
-        for (int i = 0; fused && i < n_sel; ++i) fused = sel[2 * i] != l;
-        if (fused) {
-            STB_TRY(fused_attention(q, k, v, B, H, M, T, w.attn.hi, w.attn.lo, d, 64, (long long)M * d, st));
-        } else {
-            stb_epilogue e = ep_f32(w.Sx, Tp, nullptr, nullptr, 0, 0.125f);
+        // The attention output never depends on what is captured, so the logits are the same with or without a capture.
+        STB_TRY(fused_attention(q, k, v, B, H, M, T, w.attn.hi, w.attn.lo, d, 64, (long long)M * d, st));
+        // The captured scores are their own GEMM, (q k^T) / 8 straight into qk_out; columns T..Tp-1 are not written.
+        if (qk_out != nullptr && n_sel < 0) {
+            stb_epilogue e = ep_f32(qk_out + (long long)l * H * M * Tp, Tp, nullptr, nullptr, 0, 0.125f);
             e.out_h_stride = (long long)M * Tp;
-            e.out_b_stride = (long long)H * M * Tp;
+            e.out_b_stride = (long long)n_sel_total * M * Tp;
             STB_TRY(gemm(q, k, B, H, e, st));
-            if (qk_out != nullptr) {
-                CaptureList cl;
-                cl.count = 0;
-                if (n_sel < 0) {
-                    for (int h = 0; h < H; ++h) {
-                        cl.head[cl.count] = h;
-                        cl.slot[cl.count] = l * H + h;
-                        if (++cl.count == 32) { STB_TRY(capture_heads(w.Sx, B, H, M, Tp, qk_out, n_sel_total, cl, st)); cl.count = 0; }
-                    }
-                } else {
-                    for (int i = 0; i < n_sel; ++i)
-                        if (sel[2 * i] == l) {
-                            cl.head[cl.count] = sel[2 * i + 1];
-                            cl.slot[cl.count] = i;
-                            if (++cl.count == 32) { STB_TRY(capture_heads(w.Sx, B, H, M, Tp, qk_out, n_sel_total, cl, st)); cl.count = 0; }
-                        }
-                }
-                STB_TRY(capture_heads(w.Sx, B, H, M, Tp, qk_out, n_sel_total, cl, st));
-            }
-            STB_TRY(softmax_rows(w.Sx, (long long)B * H * M, T, Tp, M, 0, w.Px.hi, w.Px.lo, Tp, st));
-            stb_operand p = opnd(w.Px.hi, w.Px.lo, M, Tp, Tp, (long long)M * Tp, (long long)H * M * Tp);
-            stb_epilogue eo = ep_split(w.attn, d, nullptr, STB_ACT_NONE, 64, (long long)M * d);
-            STB_TRY(gemm(p, v, B, H, eo, st));
+        }
+        for (int i = 0; qk_out != nullptr && i < n_sel; ++i) {
+            if (sel[2 * i] != l) continue;
+            const int h = sel[2 * i + 1];
+            stb_operand qh = opnd(offs(w.q.hi, 64 * h), offs(w.q.lo, 64 * h), M, 64, d, 0, (long long)M * d);
+            stb_operand kh = opnd(offs(Kx.hi, (long long)h * T * 64), offs(Kx.lo, (long long)h * T * 64), T, 64, 64, 0,
+                                  (long long)H * T * 64);
+            stb_epilogue e = ep_f32(qk_out + (long long)i * M * Tp, Tp, nullptr, nullptr, 0, 0.125f);
+            e.out_b_stride = (long long)n_sel * M * Tp;
+            STB_TRY(gemm(qh, kh, B, 1, e, st));
         }
         STB_TRY(linear(m, w.attn, rows, d, W_HI(L, STB_L_COUT_W), W_LO(L, STB_L_COUT_W), d,
                        ep_f32(w.x, d, W_F32(L, STB_L_COUT_B), w.x, d), st));

@@ -4,12 +4,6 @@
 
 namespace stb {
 
-struct CaptureList {          // passed by value to the capture kernel
-    int count;
-    int head[32];             // head index inside the layer
-    int slot[32];             // destination index inside qk_out's n_sel dimension
-};
-
 // cached 4-D fp16 TMA tensor map over one plane of a K-major operand view (gemm_tc.cu); perm[i] tells which of
 // (row=0, head=1, batch=2, zero=3) feeds TMA coordinate 1+i
 struct TmapVal {
@@ -31,8 +25,6 @@ int embed_tokens(const int32_t* tokens, long long n_tok, int M, int offset, int 
                  float* x, cudaStream_t st);
 int mel_repack(const float* mel, int B, int C, int T, __half* hi, __half* lo, cudaStream_t st);
 int zero_pad_rows(__half* hi, __half* lo, int B, int C, int T, cudaStream_t st);
-int capture_heads(const float* S, int B, int H, int M, long long ld, float* out, int n_sel, const CaptureList& list,
-                  cudaStream_t st);
 
 // seq_off (nullable) [B]: first cache row of each sequence (ragged initial tokens right-aligned on the shared counter)
 int decode_attn_self(const float* qkv, float* Kc, float* Vc, int B, int H, int d, int ctx, const int32_t* pos,

@@ -8,7 +8,8 @@ CPU, with the LayerNorm and softmax row kernels of those passes on their own (cs
   zero pad columns, and no read of a score outside a row's valid columns.
 - stb_encoder_forward on distinct windows (one with a silent tail, one short), with the frames where the conv padding
   enters gated on their own; stb_cross_kv (K head-major, V^T with its zero pad keys) in both layouts;
-  stb_decoder_forward logits and captured cross-attention scores for all heads and for an explicit head list.
+  stb_decoder_forward logits and captured cross-attention scores for all heads and for an explicit head list; the logits
+  bitwise the same whatever is captured, and a head list's scores bitwise those of the same heads in the all-heads pass.
 - The same passes on model-owned workspaces filled with NaN give bitwise the same outputs: every pad row, pad key and
   pad column is written before it is read.
 
@@ -78,7 +79,7 @@ def _rel(out, ref):
 @contextlib.contextmanager
 def _float64_oracle():
     """The oracle's LayerNorm casts to fp32 and its attention rounds the scores to fp32 before the softmax; keep both in
-    float64, and always return the scaled pre-softmax scores (what the cross-attention capture copies)."""
+    float64, and always return the scaled pre-softmax scores (what the cross-attention capture writes)."""
     import torch.nn.functional as F
     from oracle.whisper_ref import model as WM
 
@@ -381,7 +382,9 @@ def _decoder_inputs(c, M, seed):
                                     ("d1280", 65), ("d1280", 448)])
 def test_teacher_forced_decoder_matches_float64(cases, name, M):
     """Every logit of three distinct token rows, and the captured scaled pre-softmax cross-attention scores (columns
-    0..1499) of all heads and of an explicit head list, against the float64 decoder on this library's encoder output."""
+    0..1499) of all heads and of an explicit head list, against the float64 decoder on this library's encoder output.
+    The logits are bitwise the same with no capture, a head list or all heads; the head list's scores are bitwise those
+    of the same heads in the all-heads pass."""
     c = cases(name)
     gm = c.gm
     D = gm.dims
@@ -390,7 +393,13 @@ def test_teacher_forced_decoder_matches_float64(cases, name, M):
     ckv = gm.cross_kv(enc)
     logits, qk = gm.decode_forced(tokens, ckv, heads="all")
     _, qk_sel = gm.decode_forced(tokens, ckv, want_logits=False, heads=HEADS[name])
+    logits_none, _ = gm.decode_forced(tokens, ckv)
+    logits_sel, _ = gm.decode_forced(tokens, ckv, heads=HEADS[name])
     torch.cuda.synchronize()
+    for what, other in (("no capture", logits_none), ("a head list", logits_sel)):
+        assert torch.equal(_bits(other), _bits(logits)), f"the logits with {what} differ from those with all heads captured"
+    for i, (l, h) in enumerate(HEADS[name]):
+        assert torch.equal(_bits(qk_sel[:, i, :, :T]), _bits(qk[:, l * H + h, :, :T])), f"head list slot {i} ({l}, {h})"
     qks = [None] * D.n_text_layer
     hooks = [blk.cross_attn.register_forward_hook(lambda _m, _i, out, i=i: qks.__setitem__(i, out[-1]))
              for i, blk in enumerate(c.m64.decoder.blocks)]
