@@ -97,6 +97,8 @@ typedef struct {
     long long res_b_stride;
     float alpha;
     int act;
+    int head_cols;         /* 0, or head-major columns (row-major, n_head == 1, even): column n is stored at
+                              n / head_cols * out_h_stride + m * ld_out + n % head_cols */
 } stb_epilogue;
 
 STB_API int stb_gemm(const stb_operand* A, const stb_operand* B, int n_batch, int n_head, const stb_epilogue* ep, void* stream);

@@ -31,7 +31,7 @@ class Epilogue(ctypes.Structure):
     _fields_ = [("out_f32", c_void_p), ("out_hi", c_void_p), ("out_lo", c_void_p), ("ld_out", c_longlong),
                 ("out_h_stride", c_longlong), ("out_b_stride", c_longlong), ("transposed", c_int), ("bias", c_void_p),
                 ("bias_per_row", c_int), ("residual", c_void_p), ("ld_res", c_longlong), ("res_h_stride", c_longlong),
-                ("res_b_stride", c_longlong), ("alpha", c_float), ("act", c_int)]
+                ("res_b_stride", c_longlong), ("alpha", c_float), ("act", c_int), ("head_cols", c_int)]
 
 
 class Dims(ctypes.Structure):

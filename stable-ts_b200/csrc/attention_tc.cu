@@ -64,19 +64,6 @@ __device__ __forceinline__ uint32_t pack_h2(__half a, __half b) {
     return (uint32_t)__half_as_ushort(a) | ((uint32_t)__half_as_ushort(b) << 16);
 }
 
-// named barriers 1 and 2 (0 is __syncthreads) between the two consumer warpgroups
-template <int ID>
-__device__ __forceinline__ void named_bar_sync() { asm volatile("bar.sync %0, 256;" ::"n"(ID) : "memory"); }
-template <int ID>
-__device__ __forceinline__ void named_bar_arrive() { asm volatile("bar.arrive %0, 256;" ::"n"(ID) : "memory"); }
-
-// keeps the compiler from moving reads or writes of a wgmma accumulator across the wgmma_wait that makes it valid
-template <int N>
-__device__ __forceinline__ void fence_regs(float (&r)[N]) {
-#pragma unroll
-    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
-}
-
 template <int PASSES>
 __global__ void __launch_bounds__(AT_THREADS, 1)
 attention_tc_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUtensorMap tmQl,

@@ -212,6 +212,25 @@ __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_grou
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
+// keeps the compiler from moving reads or writes of a wgmma accumulator across the wgmma_wait that makes it valid
+template <int N>
+__device__ __forceinline__ void fence_regs(float (&r)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
+}
+
+// named barriers 1 and 2 (0 is __syncthreads) between the two consumer warpgroups of a kernel
+template <int ID>
+__device__ __forceinline__ void named_bar_sync() { asm volatile("bar.sync %0, 256;" ::"n"(ID) : "memory"); }
+template <int ID>
+__device__ __forceinline__ void named_bar_arrive() { asm volatile("bar.arrive %0, 256;" ::"n"(ID) : "memory"); }
+
+// hand registers between the warpgroups of a warp-specialised kernel (every warp of the warpgroup executes it)
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+
 // wgmma shared-memory matrix descriptor for a K-major tile whose rows are exactly 128 bytes (64 x fp16) written by TMA
 // with CU_TENSOR_MAP_SWIZZLE_128B: 8-row x 128 B swizzle atoms stacked every 1024 B (stride byte offset).  Bit layout:
 // start>>4 [0,14), LBO>>4 [16,30) (unused for swizzled K-major; 1), SBO>>4 [32,46), layout [62,64) (1 = SWIZZLE_128B).

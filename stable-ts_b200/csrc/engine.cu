@@ -105,9 +105,13 @@ static int attention(const stb_model* m, int B, int H, int d, int Mq, int Mk, in
 // V^T projection: rows of `x` (per batch item) times W_v^T, stored transposed into vT [B][H*64][ldk]
 static int project_vT(const stb_model* m, const Split& x, int B, int rows, int d, const void* w_hi, const void* w_lo,
                       const float* bias, Split vT, int ldk, cudaStream_t st) {
-    const bool lo = m->prec == STB_PREC_FP16X3;
-    STB_CUDA_OK(cudaMemsetAsync(vT.hi, 0, (size_t)B * d * ldk * sizeof(__half), st));
-    if (lo) STB_CUDA_OK(cudaMemsetAsync(vT.lo, 0, (size_t)B * d * ldk * sizeof(__half), st));
+    // The GEMM writes columns 0..rows-1.  The P.V products read the pad keys rows..ldk-1 too: their probabilities are
+    // zero, but 0 x NaN from uninitialised memory is not, so those columns are zeroed (only those: the rest is overwritten).
+    if (ldk > rows) {
+        const size_t pitch = (size_t)ldk * sizeof(__half), width = (size_t)(ldk - rows) * sizeof(__half);
+        STB_CUDA_OK(cudaMemset2DAsync(vT.hi + rows, pitch, 0, width, (size_t)B * d, st));
+        if (vT.lo) STB_CUDA_OK(cudaMemset2DAsync(vT.lo + rows, pitch, 0, width, (size_t)B * d, st));
+    }
     stb_operand a = opnd(x.hi, x.lo, rows, d, d, 0, (long long)rows * d);
     stb_operand w = opnd(w_hi, w_lo, d, d, d);
     stb_epilogue e = ep_split(vT, ldk, bias, STB_ACT_NONE, 0, (long long)d * ldk);
@@ -241,12 +245,13 @@ static int cross_kv(stb_model* m, const __half* xa_hi, const __half* xa_lo, int 
         CrossDecodeKV Vd;
         cross_ptrs(m, B, out, l, K, vT, &Vd);
         {   // K head-major [B][H][T][64] (sequential 192 KB streams per (sequence, head) for the decode-step kernel):
-            // per-head batched GEMM, A = xa broadcast over heads, B = rows h*64..h*64+63 of W_k; whisper's key has no bias
+            // one full-width GEMM whose epilogue sends column n to head n / 64; whisper's key has no bias
             const int H = D.n_text_head;
             stb_operand a = opnd(xa.hi, xa.lo, T, d, d, 0, (long long)T * d);
-            stb_operand wk = opnd(W_HI(L, STB_L_CKV_W), W_LO(L, STB_L_CKV_W), 64, d, d, 64LL * d, 0);
+            stb_operand wk = opnd(W_HI(L, STB_L_CKV_W), W_LO(L, STB_L_CKV_W), d, d, d);
             stb_epilogue e = ep_split(K, 64, nullptr, STB_ACT_NONE, (long long)T * 64, (long long)H * T * 64);
-            STB_TRY(gemm(a, wk, B, H, e, st));
+            e.head_cols = 64;
+            STB_TRY(gemm(a, wk, B, 1, e, st));
         }
         STB_TRY(project_vT(m, xa, B, T, d, offs(W_HI(L, STB_L_CKV_W), (long long)d * d), offs(W_LO(L, STB_L_CKV_W), (long long)d * d),
                            W_F32(L, STB_L_CKV_B) + d, vT, STB_KPAD, st));

@@ -10,13 +10,16 @@
 // accumulator, which reproduces an fp32 GEMM to ~1e-6 relative on the fp16 tensor pipe (the reference's CPU/align
 // path is fp32; SURVEY.md section 7 "precision vs the 1e-3 logits gate").  One pass = STB_PREC_FP16.
 //
-// Structure (PERSISTENT: one CTA per SM loops over 128 x BN output tiles; 288 threads):
-//   warps 0..3, 4..7 : two consumer warpgroups, each owns 64 rows of the tile: wgmma m64nBNk16 from the swizzled shared-memory
-//                      tiles (one group kept in flight across k-blocks), then the epilogue straight from the accumulator
-//                      fragments: bias / GELU / residual / scale -> global (fp32 row-major, split-fp16 row-major, or either
-//                      transposed)
-//   warp 8           : TMA producer (cp.async.bulk.tensor.4d, SWIZZLE_128B tiles, mbarrier complete_tx); it runs ahead into the
-//                      next tile's k-blocks while the consumers are in their epilogue
+// Structure (PERSISTENT: one CTA per SM loops over 128 x BN output tiles; 384 threads, ping-pong consumers):
+//   warpgroups 0, 1 : two consumer warpgroups; each owns whole tiles, the CTA's tiles wg, wg + 2, wg + 4, ...  Per k-block
+//                     a consumer issues wgmma m64nBNk16 for rows 0..63 and 64..127 of its tile from the swizzled shared-memory
+//                     tiles (one k-block kept in flight), then runs the epilogue straight from the accumulator fragments:
+//                     bias / GELU / residual / scale -> global (fp32 row-major, split-fp16 row-major with one 4-byte store
+//                     per plane and column pair, either transposed, or head-major column groups).  The consumers take turns
+//                     over the mainloop (named barriers), so one's epilogue runs under the other's MMAs.  setmaxnreg gives
+//                     them 232 registers (128 accumulator registers per thread at BN = 128).
+//   warpgroup 2     : one thread is the TMA producer (cp.async.bulk.tensor.4d, SWIZZLE_128B tiles, mbarrier complete_tx); it
+//                     fills the ring with the CTA's tiles in order, so a stage always belongs to one consumer
 #include <mutex>
 #include <string.h>
 #include <unordered_map>
@@ -41,6 +44,7 @@ struct GemmArgs {
     long long ld_res, res_h, res_b;
     float alpha;
     int act;
+    int head_cols;
 };
 
 template <int BN, int PASSES>
@@ -54,13 +58,102 @@ struct GemmCfg {
     static constexpr uint32_t SMEM = STAGES * STAGE + 1024;         // + slack for 1024 B alignment
 };
 
-constexpr int GEMM_THREADS = 288;    // 2 consumer warpgroups + the producer warp
+constexpr int GEMM_THREADS = 384;    // 2 consumer warpgroups + the producer warpgroup
 
 __device__ __forceinline__ void pick_coords(const int (&perm)[3], int row, int h, int b, int& c1, int& c2, int& c3) {
     int v[4] = {row, h, b, 0};      // perm id 3 = broadcast dim (stride 0): coordinate pinned to 0
     c1 = v[perm[0]];
     c2 = v[perm[1]];
     c3 = v[perm[2]];
+}
+
+// Epilogue of one 8-column fragment group, straight from the accumulator: (a0, a1) at row m, (a2, a3) at row m + 8, columns
+// n, n + 1 (n < N): bias / GELU / residual / scale -> global.
+__device__ __forceinline__ void gemm_epilogue_group(const GemmArgs& g, float a0, float a1, float a2, float a3, int m_base, int n,
+                                                    long long zo, long long zr, bool out_vec, bool res_vec, bool bias_vec,
+                                                    bool split_vec) {
+    const bool two = n + 1 < g.N;
+    // head-major columns: column n goes to head n / head_cols (stride out_h), column n % head_cols in it
+    const long long col = g.head_cols ? (long long)(n / g.head_cols) * g.out_h + n % g.head_cols : n;
+#pragma unroll
+    for (int half = 0; half < 2; ++half) {                     // fragment rows r and r + 8
+        const int m = m_base + half * 8;
+        if (m >= g.M) break;
+        float v0 = (half ? a2 : a0) * g.alpha, v1 = (half ? a3 : a1) * g.alpha;
+        if (g.bias != nullptr) {
+            if (g.bias_per_row) {
+                const float br = __ldg(g.bias + m);
+                v0 += br;
+                v1 += br;
+            } else if (two && bias_vec) {
+                const float2 bv = __ldg(reinterpret_cast<const float2*>(g.bias + n));
+                v0 += bv.x;
+                v1 += bv.y;
+            } else {
+                v0 += __ldg(g.bias + n);
+                if (two) v1 += __ldg(g.bias + n + 1);
+            }
+        }
+        if (g.act == STB_ACT_GELU) {
+            v0 = gelu_erf(v0);
+            v1 = gelu_erf(v1);
+        }
+        if (g.res != nullptr) {
+            const float* rp = g.res + zr + (long long)m * g.ld_res + n;
+            if (two && res_vec) {
+                const float2 rv = *reinterpret_cast<const float2*>(rp);
+                v0 += rv.x;
+                v1 += rv.y;
+            } else {
+                v0 += rp[0];
+                if (two) v1 += rp[1];
+            }
+        }
+        __half h0, l0, h1, l1;
+        if (g.out_hi != nullptr) {
+            split_f16(v0, h0, l0);
+            split_f16(v1, h1, l1);
+        }
+        if (!g.transposed) {
+            const long long off = zo + (long long)m * g.ld_out + col;
+            if (g.out_f32 != nullptr) {
+                if (two && out_vec) {
+                    *reinterpret_cast<float2*>(g.out_f32 + off) = make_float2(v0, v1);
+                } else {
+                    g.out_f32[off] = v0;
+                    if (two) g.out_f32[off + 1] = v1;
+                }
+            }
+            if (g.out_hi != nullptr) {
+                if (two && split_vec) {                        // one 4-byte store per plane for the column pair
+                    *reinterpret_cast<__half2*>(g.out_hi + off) = __halves2half2(h0, h1);
+                    if (g.out_lo != nullptr) *reinterpret_cast<__half2*>(g.out_lo + off) = __halves2half2(l0, l1);
+                } else {
+                    g.out_hi[off] = h0;
+                    if (two) g.out_hi[off + 1] = h1;
+                    if (g.out_lo != nullptr) {
+                        g.out_lo[off] = l0;
+                        if (two) g.out_lo[off + 1] = l1;
+                    }
+                }
+            }
+        } else {
+            // transposed store: the 8 row-lanes of a fragment column hit 8 consecutive addresses
+            const long long off = zo + (long long)n * g.ld_out + m;
+            if (g.out_f32 != nullptr) {
+                g.out_f32[off] = v0;
+                if (two) g.out_f32[off + g.ld_out] = v1;
+            }
+            if (g.out_hi != nullptr) {
+                g.out_hi[off] = h0;
+                if (two) g.out_hi[off + g.ld_out] = h1;
+                if (g.out_lo != nullptr) {
+                    g.out_lo[off] = l0;
+                    if (two) g.out_lo[off + g.ld_out] = l1;
+                }
+            }
+        }
+    }
 }
 
 template <int BN, int PASSES>
@@ -94,7 +187,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__
 #pragma unroll
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 2);                        // one arrival per consumer warpgroup
+            mbar_init(&empty_bar[s], 1);                        // a stage holds a k-block of one consumer's tile
         }
         fence_mbar_init();
     }
@@ -104,9 +197,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__
     pdl_trigger();
     pdl_wait();
 
-    if (warp == 8) {
-        // ------------------------------------------------ TMA producer
-        if (lane == 0) {
+    if (warp >= 8) {
+        // ------------------------------------------------ TMA producer (one thread), the CTA's tiles in order
+        setmaxnreg_dec<40>();
+        if (warp == 8 && lane == 0) {
             int stage = 0;
             uint32_t phase = 0;
             for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -135,26 +229,35 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__
         __syncwarp();
         return;
     }
-    // ---------------------------------------------------- consumers: warpgroup wg owns rows [64 wg, 64 wg + 64) of the tile
+    // ---------------------------------------------------- consumers: warpgroup wg owns the CTA's tiles wg, wg + 2, ...
+    setmaxnreg_inc<232>();
     const int wg = warp >> 2;
-    const uint32_t a_row_off = (uint32_t)wg * 64u * 128u;      // 8 swizzle atoms of 1024 B
-    const int frag_row = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int frag_row = (warp & 3) * 16 + (lane >> 2);
     const int frag_col = 2 * (lane & 3);
     const bool out_vec = ((g.ld_out | g.out_h | g.out_b) & 1) == 0 && (reinterpret_cast<uintptr_t>(g.out_f32) & 7) == 0;
+    const bool split_vec = ((g.ld_out | g.out_h | g.out_b) & 1) == 0 &&
+                           ((reinterpret_cast<uintptr_t>(g.out_hi) | reinterpret_cast<uintptr_t>(g.out_lo)) & 3) == 0;
     const bool res_vec = ((g.ld_res | g.res_h | g.res_b) & 1) == 0 && (reinterpret_cast<uintptr_t>(g.res) & 7) == 0;
     const bool bias_vec = (reinterpret_cast<uintptr_t>(g.bias) & 7) == 0;
-    int stage = 0;
-    uint32_t phase = 0;
-    for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        float acc[BN / 2];
+    long long j = wg;                                           // the tile's place in the CTA's sequence
+    for (long long tile = blockIdx.x + j * gridDim.x; tile < num_tiles; tile += 2LL * gridDim.x, j += 2) {
+        // the producer fills the ring in the CTA's tile order: this tile's k-blocks are ring slots j * num_kb, ...
+        const long long slot = j * num_kb;
+        int stage = (int)(slot % STAGES);
+        uint32_t phase = (uint32_t)((slot / STAGES) & 1);
+        float acc[2][BN / 2];                                   // rows 0..63 and 64..127 of the tile
 #pragma unroll
-        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        for (int i = 0; i < BN / 2; ++i) acc[0][i] = acc[1][i] = 0.f;
+        // take turns over the mainloop: wait until the other consumer has issued the previous tile's MMAs
+        if (j > 0) {
+            if (wg == 0) named_bar_sync<1>(); else named_bar_sync<2>();
+        }
         int prev_stage = -1;
         uint32_t accum = 0;
         for (int kb = 0; kb < num_kb; ++kb) {
             mbar_wait_mma(&full_bar[stage], phase);
             const uint32_t sa = smem_u32(tiles + (size_t)stage * Cfg::STAGE);
-            const uint32_t a_hi = sa + a_row_off, a_lo = a_hi + Cfg::A_TILE;
+            const uint32_t a_hi = sa, a_lo = a_hi + Cfg::A_TILE;
             const uint32_t b_hi = sa + NPL * Cfg::A_TILE, b_lo = b_hi + Cfg::B_TILE;
             wgmma_fence();
 #pragma unroll
@@ -164,7 +267,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__
                 const uint32_t pb = (pass == 1) ? b_lo : b_hi;
 #pragma unroll
                 for (int k4 = 0; k4 < 4; ++k4) {               // 4 x (K = 16 fp16 = 32 B) per 128 B swizzle row
-                    wgmma_ss(acc, wgmma_desc_k128(pa + k4 * 32), wgmma_desc_k128(pb + k4 * 32), accum);
+                    const uint64_t db = wgmma_desc_k128(pb + k4 * 32);
+                    wgmma_ss(acc[0], wgmma_desc_k128(pa + k4 * 32), db, accum);
+                    wgmma_ss(acc[1], wgmma_desc_k128(pa + 64 * 128 + k4 * 32), db, accum);   // 8 swizzle atoms on
                     accum = 1;
                 }
             }
@@ -177,96 +282,34 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__
                 phase ^= 1;
             }
         }
+        // the other consumer issues the next tile's MMAs while ours drain and this tile's epilogue runs
+        if (tile + gridDim.x < num_tiles) {
+            if (wg == 0) named_bar_arrive<2>(); else named_bar_arrive<1>();
+        }
         wgmma_wait<0>();
+        fence_regs(acc[0]);
+        fence_regs(acc[1]);
         if (prev_stage >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev_stage]);
 
-        // ------------------------------------------------ epilogue from the accumulator fragments
         const int nbk = (int)(tile % tiles_n);
         const int mbk = (int)((tile / tiles_n) % tiles_m);
         const int z = (int)(tile / ((long long)tiles_n * tiles_m));
         const int n0 = nbk * BN + frag_col, h = z % g.H, b = z / g.H;
         const long long zo = (long long)b * g.out_b + (long long)h * g.out_h;
         const long long zr = (long long)b * g.res_b + (long long)h * g.res_h;
+        // a compact loop over the column groups, the accumulator shifted down one group at a time (a few MOVs per group):
+        // unrolled, the epilogue's code outgrows the instruction cache and it runs several times slower
+#pragma unroll 1
+        for (int r = 0; r < 2; ++r) {
+#pragma unroll 1
+            for (int jj = 0; jj < BN / 8 && n0 + 8 * jj < g.N; ++jj) {
+                gemm_epilogue_group(g, acc[0][0], acc[0][1], acc[0][2], acc[0][3], mbk * 128 + 64 * r + frag_row, n0 + 8 * jj,
+                                    zo, zr, out_vec, res_vec, bias_vec, split_vec);
 #pragma unroll
-        for (int half = 0; half < 2; ++half) {                 // fragment rows r and r + 8
-            const int m = mbk * 128 + frag_row + half * 8;
-            if (m >= g.M) continue;
-            float bias_row = 0.f;
-            if (g.bias != nullptr && g.bias_per_row) bias_row = __ldg(g.bias + m);
-#pragma unroll
-            for (int j = 0; j < BN / 8; ++j) {
-                const int n = n0 + 8 * j;
-                if (n >= g.N) break;
-                const bool two = n + 1 < g.N;
-                float v0 = acc[4 * j + 2 * half] * g.alpha, v1 = acc[4 * j + 2 * half + 1] * g.alpha;
-                if (g.bias != nullptr) {
-                    if (g.bias_per_row) {
-                        v0 += bias_row;
-                        v1 += bias_row;
-                    } else if (two && bias_vec) {
-                        const float2 bv = __ldg(reinterpret_cast<const float2*>(g.bias + n));
-                        v0 += bv.x;
-                        v1 += bv.y;
-                    } else {
-                        v0 += __ldg(g.bias + n);
-                        if (two) v1 += __ldg(g.bias + n + 1);
-                    }
-                }
-                if (g.act == STB_ACT_GELU) {
-                    v0 = gelu_erf(v0);
-                    v1 = gelu_erf(v1);
-                }
-                if (g.res != nullptr) {
-                    const float* rp = g.res + zr + (long long)m * g.ld_res + n;
-                    if (two && res_vec) {
-                        const float2 rv = *reinterpret_cast<const float2*>(rp);
-                        v0 += rv.x;
-                        v1 += rv.y;
-                    } else {
-                        v0 += rp[0];
-                        if (two) v1 += rp[1];
-                    }
-                }
-                __half h0, l0, h1, l1;
-                if (g.out_hi != nullptr) {
-                    split_f16(v0, h0, l0);
-                    split_f16(v1, h1, l1);
-                }
-                if (!g.transposed) {
-                    const long long off = zo + (long long)m * g.ld_out + n;
-                    if (g.out_f32 != nullptr) {
-                        if (two && out_vec) {
-                            *reinterpret_cast<float2*>(g.out_f32 + off) = make_float2(v0, v1);
-                        } else {
-                            g.out_f32[off] = v0;
-                            if (two) g.out_f32[off + 1] = v1;
-                        }
-                    }
-                    if (g.out_hi != nullptr) {
-                        g.out_hi[off] = h0;
-                        if (two) g.out_hi[off + 1] = h1;
-                        if (g.out_lo != nullptr) {
-                            g.out_lo[off] = l0;
-                            if (two) g.out_lo[off + 1] = l1;
-                        }
-                    }
-                } else {
-                    // transposed store: the 8 row-lanes of a fragment column hit 8 consecutive addresses
-                    const long long off = zo + (long long)n * g.ld_out + m;
-                    if (g.out_f32 != nullptr) {
-                        g.out_f32[off] = v0;
-                        if (two) g.out_f32[off + g.ld_out] = v1;
-                    }
-                    if (g.out_hi != nullptr) {
-                        g.out_hi[off] = h0;
-                        if (two) g.out_hi[off + g.ld_out] = h1;
-                        if (g.out_lo != nullptr) {
-                            g.out_lo[off] = l0;
-                            if (two) g.out_lo[off + g.ld_out] = l1;
-                        }
-                    }
-                }
+                for (int i = 0; i < BN / 2 - 4; ++i) acc[0][i] = acc[0][i + 4];
             }
+#pragma unroll
+            for (int i = 0; i < BN / 2; ++i) acc[0][i] = acc[1][i];
         }
     }
 }
@@ -401,9 +444,11 @@ int gemm(const stb_operand& A, const stb_operand& B, int n_batch, int n_head, co
     STB_REQUIRE(A.hi && B.hi, "gemm: hi planes are required");
     STB_REQUIRE((A.lo != nullptr) == (B.lo != nullptr), "gemm: lo planes must be given for both operands or neither");
     STB_REQUIRE(ep.out_f32 || ep.out_hi, "gemm: no output");
+    STB_REQUIRE(ep.head_cols == 0 || (ep.head_cols > 0 && ep.head_cols % 2 == 0 && !ep.transposed && n_head == 1),
+                "gemm: head_cols must be even, row-major and with n_head == 1 (got %d)", ep.head_cols);
     const int passes = A.lo ? 3 : 1;
     const int N = B.rows;
-    // 128 x 128 is the widest tile: its accumulator is 64 registers per consumer thread, and three ring stages of the
+    // 128 x 128 is the widest tile: its accumulator is 128 registers per consumer thread, and three ring stages of the
     // four split-fp16 planes (64 KB each) fit the 227 KB of shared memory
     int BN = N <= 16 ? 16 : N <= 32 ? 32 : N <= 64 ? 64 : 128;
     if (A.rows <= 128 && n_batch * n_head == 1) {
@@ -418,7 +463,7 @@ int gemm(const stb_operand& A, const stb_operand& B, int n_batch, int n_head, co
     g.ld_out = ep.ld_out; g.out_h = ep.out_h_stride; g.out_b = ep.out_b_stride; g.transposed = ep.transposed;
     g.bias = ep.bias; g.bias_per_row = ep.bias_per_row;
     g.res = ep.residual; g.ld_res = ep.ld_res; g.res_h = ep.res_h_stride; g.res_b = ep.res_b_stride;
-    g.alpha = ep.alpha; g.act = ep.act;
+    g.alpha = ep.alpha; g.act = ep.act; g.head_cols = ep.head_cols;
     TmapVal ah, al, bh, bl;
     STB_TRY(make_tmap(A.hi, A.rows, A.k, n_head, n_batch, A.row_stride, A.h_stride, A.b_stride, 128, &ah));
     STB_TRY(make_tmap(B.hi, B.rows, B.k, n_head, n_batch, B.row_stride, B.h_stride, B.b_stride, BN, &bh));

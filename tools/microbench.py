@@ -5,6 +5,7 @@ rotating weight copies exceeds the 126 MB L2 so every launch streams its weights
     python tools/microbench.py dtw       # DTW at 16 / 64 windows x [101 x 1500]
     python tools/microbench.py step 120 4   # ms per decode step (120 windows, 4 decoder layers of large-v3 width)
     python tools/microbench.py attention # encoder attention (stb_attention) at 48 windows x 20 heads x 1500 x 1500
+    python tools/microbench.py gemm      # stb_gemm at the encoder / forced-decoder shapes of 48 large-v3 windows
 """
 import ctypes
 import json
@@ -140,6 +141,82 @@ def bench_attention(windows=48, heads=20, T=1500, iters=10):
     return res
 
 
+def bench_gemm(windows=48, iters=6):
+    """stb_gemm at the shapes one large-v3 step runs (48 windows of 1500 encoder rows, a forced decode of 229 rows per
+    window), split-fp16 operands (3 passes).  Executed TFLOP/s counts the 3 passes; the peak is the H100 SXM data
+    sheet's dense fp16 rate, not a measured one."""
+    lib = L.lib()
+    T, F, d, Tp, H = 1500, 3000, 1280, 1504, 20
+    M, Md = windows * T, windows * 229
+    g = torch.Generator(device="cuda").manual_seed(0)
+
+    def split(*shape, scale=1.0):
+        x = torch.randn(*shape, device="cuda", generator=g) * scale
+        h = x.half()
+        return h, (x - h.float()).half()
+
+    def zeros(n, dt=torch.float16):
+        return torch.zeros(n, dtype=dt, device="cuda")
+
+    res = {"card": _card(), "windows": windows, "peak_tflops": 989.0,
+           "peak_source": "H100 SXM data sheet, dense fp16 at 700 W (not measured)", "runs": []}
+    xh, xl = split(M, 4 * d)                 # large enough for every A operand below (fc2's K = 5120)
+    wh, wl = split(51866, d, scale=0.03)     # large enough for every weight below (logits' 51866 rows)
+    bias = torch.randn(51866, device="cuda", generator=g)
+    out_h, out_l = zeros(M * 4 * d), zeros(M * 4 * d)
+    out_f = zeros(max(M * d, Md * 51872), torch.float32)
+
+    def op(hi, lo, rows, k, rs, hs=0, bs=0):
+        return L.Operand(L.ptr(hi), L.ptr(lo), rows, k, rs, hs, bs)
+
+    def ep(ld, split_out=True, f32=False, res_=False, act=0, bias_=True, transposed=False, out_h_stride=0, out_b=0,
+           res_b=None):
+        e = L.Epilogue()
+        if split_out:
+            e.out_hi, e.out_lo = L.ptr(out_h), L.ptr(out_l)
+        if f32:
+            e.out_f32 = L.ptr(out_f)
+        e.ld_out, e.out_h_stride, e.out_b_stride, e.transposed = ld, out_h_stride, out_b, int(transposed)
+        e.bias = L.ptr(bias) if bias_ else None
+        if res_:
+            e.residual, e.ld_res = L.ptr(out_f), ld
+            e.res_b_stride = out_b if res_b is None else res_b
+        e.alpha, e.act = 1.0, act
+        return e
+
+    A1280 = op(xh, xl, M, d, d)
+    Ab = op(xh, xl, T, d, d, 0, T * d)                     # per-window view (batch stride T rows)
+    cases = [
+        ("enc q|k", A1280, op(wh, wl, 2 * d, d, d), 1, 1, ep(2 * d), M, 2 * d, d),
+        ("enc V^T", Ab, op(wh, wl, d, d, d), windows, 1, ep(Tp, transposed=True, out_b=d * Tp), M, d, d),
+        ("enc out", A1280, op(wh, wl, d, d, d), 1, 1, ep(d, split_out=False, f32=True, res_=True), M, d, d),
+        ("enc fc1", A1280, op(wh, wl, 4 * d, d, d), 1, 1, ep(4 * d, act=1), M, 4 * d, d),
+        ("enc fc2", op(xh, xl, M, 4 * d, 4 * d), op(wh, wl, d, 4 * d, 4 * d), 1, 1,
+         ep(d, split_out=False, f32=True, res_=True), M, d, 4 * d),
+        ("enc conv2", op(xh, xl, T, 3 * d, 2 * d, 0, (F + 2) * d), op(wh, wl, d, 3 * d, 3 * d), windows, 1,
+         ep(d, split_out=False, f32=True, res_=True, act=1, out_b=T * d, res_b=0), M, d, 3 * d),
+        ("cross K per-head", Ab, op(wh, wl, 64, d, d, 64 * d, 0), windows, H,
+         ep(64, bias_=False, out_h_stride=T * 64, out_b=H * T * 64), M, d, d),
+        ("dec fc1", op(xh, xl, Md, d, d), op(wh, wl, 4 * d, d, d), 1, 1, ep(4 * d, act=1), Md, 4 * d, d),
+        ("dec logits", op(xh, xl, Md, d, d), op(wh, wl, 51866, d, d), 1, 1,
+         ep(51872, split_out=False, f32=True, bias_=False), Md, 51866, d),
+    ]
+    if any(f == "head_cols" for f, _ in L.Epilogue._fields_):
+        e = ep(64, bias_=False, out_h_stride=T * 64, out_b=H * T * 64)
+        e.head_cols = 64
+        cases.insert(7, ("cross K head-major", Ab, op(wh, wl, d, d, d), windows, 1, e, M, d, d))
+    for name, a, b, nb, nh, e, m, n, k in cases:
+        def run(i, a=a, b=b, nb=nb, nh=nh, e=e):
+            L.check(lib.stb_gemm(ctypes.byref(a), ctypes.byref(b), nb, nh, ctypes.byref(e), L.stream_ptr()))
+        us = _time(run, iters)
+        tf = 3 * 2.0 * m * n * k / (us * 1e-6) / 1e12
+        res["runs"].append(dict(shape=name, M=m, N=n, K=k, us=round(us, 1), executed_tflops=round(tf, 1),
+                                executed_frac_of_peak=round(tf / 989.0, 3)))
+        print(res["runs"][-1], flush=True)
+    print(res["card"], flush=True)
+    return res
+
+
 def bench_step(windows=120, layers=4, s1=24, s2=72):
     """ms per KV-cached decode step of a large-v3-WIDTH model with `layers` decoder layers (cross K/V of 120 windows x 32
     layers would not leave room for A/B runs), from the slope between two forced decodes of s1 and s2 steps (graph replay):
@@ -188,5 +265,5 @@ if __name__ == "__main__":
     elif what == "ncu":          # short run for `ncu -k regex:...`: fc1 / fc2 at 64 sequences + one DTW batch
         res = [bench_gemv((64,), ((5120, 1280), (1280, 5120)), iters=4), bench_dtw((16,))]
     else:
-        res = {"gemv": bench_gemv, "dtw": bench_dtw, "attention": bench_attention}[what]()
+        res = {"gemv": bench_gemv, "dtw": bench_dtw, "attention": bench_attention, "gemm": bench_gemm}[what]()
     print(json.dumps({what: res, "env": {k: v for k, v in os.environ.items() if k.startswith("STB_")}}))
