@@ -1,7 +1,8 @@
 """``load_model`` and the bound model methods (mirror of stable_whisper/whisper_word_level/original_whisper.py:931-1009).
 
 ``load_model`` returns a ``B200Whisper`` on which ``modify_model`` has bound ``transcribe`` / ``align`` / ``align_words`` /
-``refine`` / ``locate`` -- the names the reference binds at original_whisper.py:942-949 -- each returning a WhisperResult
+``refine`` / ``locate`` -- the names the reference binds at original_whisper.py:942-949 -- and ``transcribe_batch`` (many
+recordings through shared device batches, one result each), each returning a WhisperResult
 (``result.make_result``: the reference's own class when ``stable_whisper`` is importable, else the schema-compatible
 stand-in of ``result.py``).
 
@@ -227,51 +228,113 @@ def _set_language(result, tokenizer, language):
     return result
 
 
-def transcribe(model: B200Whisper, audio, *, language: Optional[str] = None, task: str = "transcribe", word_timestamps: bool = True,
-               regroup=True, suppress_silence: bool = True, suppress_word_ts: bool = True, use_word_position: bool = True,
-               nonspeech_error: float = 0.1, suppress_ts_tokens: bool = False, q_levels: int = 20, k_size: int = 5,
-               temperature: Union[float, Tuple[float, ...]] = (0.0, 0.2, 0.4, 0.6, 0.8, 1.0),
-               compression_ratio_threshold: Optional[float] = 2.4, no_speech_threshold: Optional[float] = 0.6,
-               logprob_threshold: Optional[float] = -1.0, condition_on_previous_text: bool = True,
-               initial_prompt: Optional[str] = None, max_instant_words: Optional[float] = 0.5, gap_padding: str = " ...",
-               min_word_dur: float = 0.1, batch_windows: int = 16, shard_seconds: Optional[float] = 30.0, tokenizer=None,
-               nonspeech_skip: Optional[float] = None, avg_prob_threshold: Optional[float] = None, clip_timestamps=None,
-               dynamic_heads=None, aligner="legacy", extra_models=None, prepend_punctuations: Optional[str] = None,
-               append_punctuations: Optional[str] = None, split_callback=None, progress_callback=None,
-               verbose: Optional[bool] = False, ignore_compatibility: bool = False, only_voice_freq: bool = False,
-               generator: Optional[torch.Generator] = None, uniforms=None, **decode_options):
-    """``model.transcribe`` (transcribe_stable, original_whisper.py:27-78): -> WhisperResult.  Static 30 s shards batched
-    ``batch_windows`` at a time (transcribe.py); ``shard_seconds=None`` walks the audio as one sequential shard like the
-    reference.  Decoding defaults are the reference's: the temperature fallback sequence with its compression-ratio /
-    log-prob / no-speech tests, ``best_of`` draws at temperature > 0, the previous window's text as the prompt of the next
-    (inside a shard).  ``suppress_silence``: as in the reference (original_whisper.py:428) the non-VAD silence detector only
-    runs when it is True -- silent windows are then skipped and ``suppress_ts_tokens`` masks the silent timestamp tokens.  The
-    word re-timing against the detected silences (``Segment.suppress_silence``, result.py; governed by ``suppress_word_ts`` /
+def _detect_languages(model: B200Whisper, waves, batch_windows: int):
+    """``model.detect_language_of(wave[:480000])`` of every waveform, with up to ``batch_windows`` first 30 s per log-mel /
+    encoder / language-token pass.  A shorter first 30 s is zero-filled up to the longest one of its batch: the log-mel
+    zero-pads every row to 30 s anyway, so a row's mel -- and with it the encoder and decoder rows -- is the one it gets alone."""
+    found = []
+    step = max(int(batch_windows), 1)
+    for lo in range(0, len(waves), step):
+        heads = [w[:480000] for w in waves[lo:lo + step]]
+        rows = torch.zeros(len(heads), max(int(h.numel()) for h in heads))
+        for b, h in enumerate(heads):
+            rows[b, : h.numel()] = h
+        _, probs = model.detect_language(model.log_mel(rows.to(model.device)))
+        found += [max(p, key=p.get) for p in probs]
+    return found
+
+
+def transcribe(model: B200Whisper, audio, *, language: Optional[str] = None, initial_prompt: Optional[str] = None, **options):
+    """``model.transcribe`` (transcribe_stable, original_whisper.py:27-78): -> WhisperResult.  The one-recording case of
+    ``transcribe_batch``; every option and its default is listed at ``_transcribe``."""
+    return _transcribe(model, [audio], [language], [initial_prompt], **options)[0]
+
+
+def transcribe_batch(model: B200Whisper, audios, *, language=None, initial_prompt=None, **options):
+    """``model.transcribe_batch``: many recordings -> one WhisperResult per recording, in input order.
+
+    Every recording's windows join one queue of device batches (transcribe.transcribe_recordings), so short recordings share
+    decode steps instead of each running at batch 1.  ``audios``: a sequence of anything ``transcribe`` takes (path, bytes,
+    ndarray, tensor).  ``language`` / ``initial_prompt``: one value for every recording or a list with one entry per
+    recording; ``None`` in a ``language`` list detects that recording's language (on its first 30 s, batched).  Recordings of
+    different languages never share a decode batch.  Every other option is shared and means what it means in ``transcribe``;
+    ``progress_callback`` counts over all recordings.  ``clip_timestamps`` is refused (one clip list means nothing across
+    different recordings), and so is ``tokenizer`` together with a language list.
+
+    ``transcribe_batch(audios, **kw)[i]`` equals ``transcribe(audios[i], **kw_i)``, ``kw_i`` being ``kw`` with that recording's
+    language and initial prompt -- segments, seeks, tokens and word times, word probabilities up to the decode-step route
+    that the batch size selects -- as long as no window falls back to a temperature above 0: the draws of such windows come
+    from the shared ``generator`` / ``uniforms`` stream in batch order."""
+    audios = list(audios)
+
+    def per_recording(name, value):
+        if not isinstance(value, (list, tuple)):
+            return [value] * len(audios)
+        if len(value) != len(audios):
+            raise ValueError(f"transcribe_batch: {len(value)} entries in {name} for {len(audios)} recordings")
+        return list(value)
+    if options.get("clip_timestamps") is not None:
+        raise TypeError("transcribe_batch does not take clip_timestamps (one clip list means nothing across recordings)")
+    if options.get("tokenizer") is not None and isinstance(language, (list, tuple)):
+        raise ValueError("transcribe_batch: pass either tokenizer= or a per-recording language list, not both")
+    return _transcribe(model, audios, per_recording("language", language), per_recording("initial_prompt", initial_prompt),
+                       **options)
+
+
+def _transcribe(model: B200Whisper, audios, languages, initial_prompts, *, task: str = "transcribe",
+                word_timestamps: bool = True, regroup=True, suppress_silence: bool = True, suppress_word_ts: bool = True,
+                use_word_position: bool = True, nonspeech_error: float = 0.1, suppress_ts_tokens: bool = False,
+                q_levels: int = 20, k_size: int = 5, temperature: Union[float, Tuple[float, ...]] = (0.0, 0.2, 0.4, 0.6, 0.8, 1.0),
+                compression_ratio_threshold: Optional[float] = 2.4, no_speech_threshold: Optional[float] = 0.6,
+                logprob_threshold: Optional[float] = -1.0, condition_on_previous_text: bool = True,
+                max_instant_words: Optional[float] = 0.5, gap_padding: str = " ...", min_word_dur: float = 0.1,
+                batch_windows: int = 16, shard_seconds: Optional[float] = 30.0, tokenizer=None,
+                nonspeech_skip: Optional[float] = None, avg_prob_threshold: Optional[float] = None, clip_timestamps=None,
+                dynamic_heads=None, aligner="legacy", extra_models=None, prepend_punctuations: Optional[str] = None,
+                append_punctuations: Optional[str] = None, split_callback=None, progress_callback=None,
+                verbose: Optional[bool] = False, ignore_compatibility: bool = False, only_voice_freq: bool = False,
+                generator: Optional[torch.Generator] = None, uniforms=None, **decode_options):
+    """``transcribe`` / ``transcribe_batch`` over recordings ``audios`` with one language (None: detect) and one initial
+    prompt each -> one WhisperResult per recording.  Static 30 s shards batched ``batch_windows`` at a time
+    (transcribe.py); ``shard_seconds=None`` walks each recording as one sequential shard like the reference.  Decoding
+    defaults are the reference's: the temperature fallback sequence with its compression-ratio / log-prob / no-speech tests,
+    ``best_of`` draws at temperature > 0, the previous window's text as the prompt of the next (inside a shard).
+    ``suppress_silence``: as in the reference (original_whisper.py:428) the non-VAD silence detector only runs when it is
+    True -- silent windows are then skipped and ``suppress_ts_tokens`` masks the silent timestamp tokens.  The word
+    re-timing against the detected silences (``Segment.suppress_silence``, result.py; governed by ``suppress_word_ts`` /
     ``use_word_position`` / ``nonspeech_error``) is the reference's own code: it is applied per window exactly where the
     reference applies it (original_whisper.py:677-689) when stable-ts is installed, and skipped -- with a warning -- when it is
-    not (result post-processing is outside this package's scope).  ``generator`` / ``uniforms``: random stream of the temperature > 0 passes (decode.decode_with_fallback).
-    Beam search is not implemented.  ``progress_callback(seconds_done, total_seconds)`` as in the reference; ``verbose=True``
-    prints the segments; ``ignore_compatibility`` is accepted for call compatibility (there is no whisper version to check).
+    not (result post-processing is outside this package's scope).  ``generator`` / ``uniforms``: random stream of the
+    temperature > 0 passes (decode.decode_with_fallback).  Beam search is not implemented.
+    ``progress_callback(seconds_done, total_seconds)`` as in the reference; ``verbose=True`` prints the segments;
+    ``ignore_compatibility`` is accepted for call compatibility (there is no whisper version to check).
     ``only_voice_freq``: band-limit the waveform to 200-5000 Hz first (audio_io.voice_freq_filter), so that language
-    detection, the silence detector, the log-mel and the decode all see the filtered audio, as in the reference."""
+    detection, the silence detector, the log-mel and the decode all see the filtered audio, as in the reference.
+    A multilingual model detects the language of every recording without one on its first 30 s (``_detect_languages``)."""
     from .decode import DecodingOptions
     from .tokenizer import get_tokenizer
-    from .transcribe import transcribe as run
+    from .transcribe import transcribe_recordings
     if decode_options.get("beam_size") is not None:
         raise NotImplementedError("H100 transcribe: beam search is not implemented (greedy / temperature sampling only)")
     if decode_options.pop("prompt", None):
         raise TypeError("transcribe: use initial_prompt (the per-window prompt is managed by condition_on_previous_text)")
-    wave = _as_waveform(audio, model)
+    waves = [_as_waveform(audio, model) for audio in audios]
     if only_voice_freq:
-        wave = _voice_freq(wave, model)
-    if language is None:
-        language = "en" if not model.is_multilingual else model.detect_language_of(wave[:480000])
-    tk = tokenizer or get_tokenizer(model, language=language, task=task, synthetic=getattr(model, "random_init", False))
+        waves = [_voice_freq(wave, model) for wave in waves]
+    languages = [lang if lang is not None or model.is_multilingual else "en" for lang in languages]
+    undetected = [r for r, lang in enumerate(languages) if lang is None]
+    for r, lang in zip(undetected, _detect_languages(model, [waves[r] for r in undetected], batch_windows)):
+        languages[r] = lang
+    tokenizers = {}                                    # one per language: the scheduler batches recordings that share one
+    for lang in languages:
+        if lang not in tokenizers:
+            tokenizers[lang] = tokenizer or get_tokenizer(model, language=lang, task=task,
+                                                          synthetic=getattr(model, "random_init", False))
     unknown = sorted(k for k in decode_options if k not in DecodingOptions.__dataclass_fields__)
     if unknown:                                        # the reference hands them to DecodingOptions(**kwargs), which raises too
         raise TypeError(f"transcribe() got unexpected decoding option(s): {unknown}")
-    opts = DecodingOptions(task=task, language=language, max_initial_timestamp=decode_options.pop("max_initial_timestamp", None),
-                           **decode_options)
+    opts = DecodingOptions(task=task, language=languages[0] if languages else None,
+                           max_initial_timestamp=decode_options.pop("max_initial_timestamp", None), **decode_options)
     hook = None
     if suppress_silence and word_timestamps:
         try:
@@ -284,25 +347,28 @@ def transcribe(model: B200Whisper, audio, *, language: Optional[str] = None, tas
         except Exception:
             warnings.warn("stable-ts is not installed: the words are not re-timed against the detected silences "
                           "(suppress_silence only gates the silence detector here)")
-    d = run(model, tk, wave, batch_windows=batch_windows, shard_seconds=shard_seconds, word_timestamps=word_timestamps,
-            options=opts, suppress_ts_tokens=bool(suppress_ts_tokens and suppress_silence), skip_silent=bool(suppress_silence),
-            q_levels=q_levels, k_size=k_size,
-            no_speech_threshold=no_speech_threshold, logprob_threshold=logprob_threshold, max_instant_words=max_instant_words,
-            gap_padding=gap_padding, min_word_dur=min_word_dur, temperature=temperature,
-            compression_ratio_threshold=compression_ratio_threshold, condition_on_previous_text=condition_on_previous_text,
-            initial_prompt=initial_prompt, generator=generator, uniforms=uniforms,
-            nonspeech_skip=nonspeech_skip if suppress_silence else None, avg_prob_threshold=avg_prob_threshold,
-            clip_timestamps=clip_timestamps, segment_hook=hook, dynamic_heads=dynamic_heads, aligner=aligner,
-            extra_models=extra_models, prepend_punctuations=prepend_punctuations, append_punctuations=append_punctuations,
-            split_callback=split_callback, progress_callback=progress_callback)
-    d["language"] = language
-    if verbose:                                        # the reference prints every segment as it is produced; here at the end
-        for sg in d["segments"]:
-            print(f"[{sg['start']:.3f} --> {sg['end']:.3f}] {sg['text']}")
-    res = make_result(d)
-    if regroup and hasattr(res, "regroup") and word_timestamps:
-        res.regroup(regroup)
-    return res
+    done = transcribe_recordings(
+        model, [tokenizers[lang] for lang in languages], waves, initial_prompts=initial_prompts, batch_windows=batch_windows,
+        shard_seconds=shard_seconds, word_timestamps=word_timestamps, options=opts,
+        suppress_ts_tokens=bool(suppress_ts_tokens and suppress_silence), skip_silent=bool(suppress_silence),
+        q_levels=q_levels, k_size=k_size, no_speech_threshold=no_speech_threshold, logprob_threshold=logprob_threshold,
+        max_instant_words=max_instant_words, gap_padding=gap_padding, min_word_dur=min_word_dur, temperature=temperature,
+        compression_ratio_threshold=compression_ratio_threshold, condition_on_previous_text=condition_on_previous_text,
+        generator=generator, uniforms=uniforms, nonspeech_skip=nonspeech_skip if suppress_silence else None,
+        avg_prob_threshold=avg_prob_threshold, clip_timestamps=clip_timestamps, segment_hook=hook,
+        dynamic_heads=dynamic_heads, aligner=aligner, extra_models=extra_models, prepend_punctuations=prepend_punctuations,
+        append_punctuations=append_punctuations, split_callback=split_callback, progress_callback=progress_callback)
+    results = []
+    for d, lang in zip(done, languages):
+        d["language"] = lang
+        if verbose:                                    # the reference prints every segment as it is produced; here at the end
+            for sg in d["segments"]:
+                print(f"[{sg['start']:.3f} --> {sg['end']:.3f}] {sg['text']}")
+        res = make_result(d)
+        if regroup and hasattr(res, "regroup") and word_timestamps:
+            res.regroup(regroup)
+        results.append(res)
+    return results
 
 
 def align(model: B200Whisper, audio, text, language: Optional[str] = None, *, tokenizer=None, remove_instant_words: bool = False,
@@ -411,6 +477,7 @@ def modify_model(model: B200Whisper) -> B200Whisper:
     """Bind the user-facing methods on the model object, as the reference does (original_whisper.py:931-949)."""
     model.transcribe = MethodType(transcribe, model)
     model.transcribe_minimal = MethodType(transcribe, model)
+    model.transcribe_batch = MethodType(transcribe_batch, model)
     model.align = MethodType(align, model)
     model.align_words = MethodType(align_words, model)
     model.refine = MethodType(refine, model)

@@ -21,6 +21,7 @@ mirrored too; ``only_voice_freq`` is applied by ``api.transcribe`` to the whole 
 regrouping, and the word-level ``suppress_silence`` re-timing of result.py -- for which ``transcribe(segment_hook=...)`` takes
 the reference's own class.
 """
+from dataclasses import replace
 from typing import List, Optional, Sequence
 
 import numpy as np
@@ -239,20 +240,34 @@ def clip_sections(clip_timestamps, total: int) -> List[List[int]]:
     return out
 
 
-def transcribe(model: B200Whisper, tokenizer, audio: torch.Tensor, *, batch_windows: int = 16, shard_seconds: Optional[float] = 30.0,
-               no_speech_threshold: Optional[float] = 0.6, logprob_threshold: Optional[float] = -1.0,
-               max_instant_words: Optional[float] = 0.5, skip_silent: bool = True, condition_on_previous_text: bool = False,
-               initial_prompt: Optional[str] = None, clip_timestamps=None, segment_hook=None, progress_callback=None,
-               **kw) -> dict:
-    """One long audio as static shards (clip boundaries at multiples of ``shard_seconds``, no prompt carry-over: the sharded
-    setting of SURVEY.md section 8e).  Inside a shard the walk is the reference's: a window starts at the shard's seek,
-    and the seek then moves by the data-dependent amount of original_whisper.py:703-710, so the tail after the last closed
-    segment of a window is decoded again by the next window.  Every round batches the current window of up to
-    ``batch_windows`` unfinished shards.  ``shard_seconds=None``: the whole audio is one shard (sequential, as the reference).
-    condition_on_previous_text / initial_prompt: the tokens of a shard's kept segments are the prompt of its next window
+def transcribe(model: B200Whisper, tokenizer, audio: torch.Tensor, *, initial_prompt: Optional[str] = None, **kw) -> dict:
+    """One audio: the one-recording case of ``transcribe_recordings`` (see there for every option).
+    -> dict(text, segments, language) in the shape of WhisperResult.to_dict (result.py:1398-1406)."""
+    return transcribe_recordings(model, [tokenizer], [audio], initial_prompts=[initial_prompt], **kw)[0]
+
+
+def transcribe_recordings(model: B200Whisper, tokenizers: Sequence, audios: Sequence[torch.Tensor], *,
+                          initial_prompts: Optional[Sequence[Optional[str]]] = None, batch_windows: int = 16,
+                          shard_seconds: Optional[float] = 30.0, no_speech_threshold: Optional[float] = 0.6,
+                          logprob_threshold: Optional[float] = -1.0, max_instant_words: Optional[float] = 0.5,
+                          skip_silent: bool = True, condition_on_previous_text: bool = False, clip_timestamps=None,
+                          segment_hook=None, progress_callback=None, options: Optional[DecodingOptions] = None,
+                          **kw) -> List[dict]:
+    """Several audios, each with its own tokenizer and initial prompt, as static shards in one queue.
+
+    Every audio is cut into static shards (clip boundaries at multiples of ``shard_seconds``, no prompt carry-over: the
+    sharded setting of SURVEY.md section 8e).  Inside a shard the walk is the reference's: a window starts at the shard's
+    seek, and the seek then moves by the data-dependent amount of original_whisper.py:703-710, so the tail after the last
+    closed segment of a window is decoded again by the next window.  Every round takes the tokenizer of the first unfinished
+    shard in the queue and batches the current window of up to ``batch_windows`` unfinished shards that share that tokenizer
+    (the caller builds one tokenizer per language, so audios in different languages never share a decode batch); shards that
+    are not finished go back to the front of the queue.  ``shard_seconds=None``: every audio is one shard (sequential, as the
+    reference).  A shard's windows depend only on that shard, so every audio's result equals the one it gets alone, except
+    that temperature > 0 draws come from the shared ``generator`` / ``uniforms`` stream in batch order.
+    condition_on_previous_text / initial_prompts: the tokens of a shard's kept segments are the prompt of its next window
     (``all_tokens[prompt_reset_since:]``, original_whisper.py:320-323,533,673-675,696-698), reset after a window decoded at
-    temperature > 0.5; every shard starts from ``initial_prompt``.
-    clip_timestamps: only these [start, end) sections are transcribed (the reference's ``load_sections``,
+    temperature > 0.5; every shard starts from its audio's initial prompt.
+    clip_timestamps: only these [start, end) sections of every audio are transcribed (the reference's ``load_sections``,
     audio/__init__.py:414-429: a window never crosses a section end, and a section is left once ``seek + 1 >= end``).  With
     ``shard_seconds=None`` they are walked in order as ONE shard (shared prompt state, exactly the reference); otherwise every
     clip is a shard of its own and the clips run batched side by side.
@@ -260,19 +275,26 @@ def transcribe(model: B200Whisper, tokenizer, audio: torch.Tensor, *, batch_wind
     silences were detected -- where ``api.transcribe`` plugs the reference's own ``Segment.suppress_silence`` re-timing
     (original_whisper.py:677-689) when stable-ts is installed.
     progress_callback(seconds_done, total_seconds): called after every round of windows (the reference's callback,
-    original_whisper.py:480-481; with several shards in flight ``seconds_done`` is the audio covered over all shards).
-    -> dict(text, segments, language) in the shape of WhisperResult.to_dict (result.py:1398-1406)."""
-    audio = audio.detach().float().flatten()
-    total = int(audio.numel())
-    # a shard = a list of [start, end) sections walked in order + the index of the current one + the seek inside it
-    if clip_timestamps:
-        secs = [sc for sc in clip_sections(clip_timestamps, total)]
-        plans = [secs] if not shard_seconds else [[sc] for sc in secs]
-        slack = 1                                                        # `seek + 1 >= max_seek` ends a section
-    else:
-        step = total if not shard_seconds else max(int(round(shard_seconds * SAMPLE_RATE)), 1)
-        plans = [[[lo, min(lo + step, total)]] for lo in range(0, max(total, 1), step)]
-        slack = 0
+    original_whisper.py:480-481; with several shards in flight ``seconds_done`` is the audio covered over all shards of all
+    audios).
+    -> one dict(text, segments, language) per audio, in the shape of WhisperResult.to_dict (result.py:1398-1406); segment
+    ``id``s count per audio."""
+    audios = [a.detach().float().flatten() for a in audios]
+    initial_prompts = list(initial_prompts) if initial_prompts is not None else [None] * len(audios)
+    # a shard = the audio it belongs to + a list of [start, end) sections walked in order + the index of the current one +
+    # the seek inside it
+    rec, plans = [], []
+    slack = 1 if clip_timestamps else 0                                  # `seek + 1 >= max_seek` ends a section
+    for r, audio in enumerate(audios):
+        total = int(audio.numel())
+        if clip_timestamps:
+            secs = clip_sections(clip_timestamps, total)
+            own = [secs] if not shard_seconds else [[sc] for sc in secs]
+        else:
+            step = total if not shard_seconds else max(int(round(shard_seconds * SAMPLE_RATE)), 1)
+            own = [[[lo, min(lo + step, total)]] for lo in range(0, max(total, 1), step)]
+        rec += [r] * len(own)
+        plans += own
     cur = [0] * len(plans)                                               # current section of every shard
     seek = [p[0][0] if p else 0 for p in plans]
 
@@ -289,15 +311,19 @@ def transcribe(model: B200Whisper, tokenizer, audio: torch.Tensor, *, batch_wind
     per_shard = [[] for _ in plans]
     covered = [0] * len(plans)                                           # samples walked per shard (progress reporting)
     span = max(sum(hi - lo for p in plans for lo, hi in p), 1)
-    init = tokenizer.encode(" " + initial_prompt.strip()) if initial_prompt is not None else []
-    all_tokens = [list(init) for _ in plans]
+    inits = [tokenizers[r].encode(" " + p.strip()) if p is not None else [] for r, p in enumerate(initial_prompts)]
+    all_tokens = [list(inits[r]) for r in rec]
     reset_since = [0] * len(plans)
-    use_prompts = condition_on_previous_text or bool(init)
+    use_prompts = condition_on_previous_text or any(inits)
     live = [i for i in range(len(plans)) if plans[i] and settle(i)]
     while live:
-        now, live = live[:batch_windows], live[batch_windows:]
-        part = [audio[seek[i]: min(seek[i] + N_SAMPLES, plans[i][cur[i]][1])] for i in now]
-        segs, info = transcribe_windows(model, tokenizer, part, time_offsets=[seek[i] / SAMPLE_RATE for i in now],
+        tk = tokenizers[rec[live[0]]]
+        now = [i for i in live if tokenizers[rec[i]] is tk][:batch_windows]
+        taken = set(now)
+        live = [i for i in live if i not in taken]
+        part = [audios[rec[i]][seek[i]: min(seek[i] + N_SAMPLES, plans[i][cur[i]][1])] for i in now]
+        opts = options if options is None else replace(options, language=getattr(tk, "language", None) or options.language)
+        segs, info = transcribe_windows(model, tk, part, time_offsets=[seek[i] / SAMPLE_RATE for i in now], options=opts,
                                         no_speech_threshold=no_speech_threshold, logprob_threshold=logprob_threshold,
                                         max_instant_words=max_instant_words, skip_silent=skip_silent,
                                         prompts=[all_tokens[i][reset_since[i]:] for i in now] if use_prompts else None, **kw)
@@ -318,8 +344,11 @@ def transcribe(model: B200Whisper, tokenizer, audio: torch.Tensor, *, batch_wind
         live = again + live
         if progress_callback is not None:
             progress_callback(round(min(sum(covered), span) / SAMPLE_RATE, 2), round(span / SAMPLE_RATE, 2))
-    segments = [s for ps in per_shard for s in ps]
-    for k, s in enumerate(segments):
-        s["id"] = k
-    return dict(text="".join(s["text"] for s in segments), segments=segments,
-                language=getattr(tokenizer, "language", None) or "en")
+    out = []
+    for r, tokenizer in enumerate(tokenizers):
+        segments = [s for i, ps in enumerate(per_shard) if rec[i] == r for s in ps]
+        for k, s in enumerate(segments):
+            s["id"] = k
+        out.append(dict(text="".join(s["text"] for s in segments), segments=segments,
+                        language=getattr(tokenizer, "language", None) or "en"))
+    return out
