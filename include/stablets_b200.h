@@ -356,9 +356,12 @@ typedef struct {
  *   ts_mask (nullable) uint8 silent-timestamp mask: [1501] shared by the batch (ts_mask_stride = 0) or one row per
  *   sequence [B][ts_mask_stride] (the reference computes one per window, original_whisper.py:504-511), NaN -> -inf, argmax (first max index), log-softmax gather,
  *   sum_logprob += logprob unless the sequence already ended, ended sequences keep emitting EOT.
+ *   Timestamp rule ("timestamps outweigh text"): skipped for a row that still holds a NaN after the filters' masks, as the
+ *   reference's log_softmax of such a row is all NaN and suppresses no text.  A masked NaN is overwritten with -inf first.
  *   Step tables (nullable, [table_rows][B] int32, row = n_sampled so no per-step host traffic is needed):
  *   forced_table: token appended instead of the argmax (fixed-length benchmark scripts / teacher forcing);
- *   token_table: the appended token; argmax_table: the argmax before forcing.  next_out [B] feeds stb_decode_step. */
+ *   token_table: the appended token; argmax_table: the argmax before forcing.  next_out [B] feeds stb_decode_step.
+ *   A step at n_sampled >= table_rows writes no table entry, reads no forced token and no uniform, and appends the argmax. */
 STB_API int stb_sample_greedy(float* logits, long long ld, int B, int V, int eot, int ts_begin, int no_timestamps,
                       const uint8_t* suppress_mask, const uint8_t* first_step_mask, const uint8_t* ts_mask,
                       long long ts_mask_stride, int max_initial_ts, int apply_ts_rules, const int32_t* forced_table, stb_seq_state* states,

@@ -427,6 +427,7 @@ sample_greedy_kernel(float* __restrict__ logits, long long ld, int V, int eot, i
     if (apply_ts_rules && st.last_ts >= 0) ts_floor = (last_ts && !penult_ts) ? st.last_ts : st.last_ts + 1;
     // ---- pass 1: SuppressBlank / SuppressTokens / ApplyTimestampRules masks; max over text / timestamp ranges
     float mx_text = -INFINITY, mx_ts = -INFINITY;
+    int has_nan = 0;                                        // an unmasked NaN anywhere in the row
     for (int i = threadIdx.x; i < V; i += blockDim.x) {
         float v = l[i];
         bool kill = (suppress && suppress[i]) || (first && first_mask && first_mask[i]);
@@ -444,12 +445,16 @@ sample_greedy_kernel(float* __restrict__ logits, long long ld, int V, int eot, i
         }
         if (kill) v = -INFINITY;
         l[i] = v;
+        has_nan |= v != v;
         if (i < ts_begin) mx_text = fmaxf(mx_text, v); else mx_ts = fmaxf(mx_ts, v);
     }
     mx_text = block_max(mx_text, red);
     mx_ts = block_max(mx_ts, red);
+    // the reference's fp32 log_softmax turns a row holding a NaN into NaN everywhere, so `ts_lp > max_text_lp` is False
+    // and no text is suppressed; fmaxf above skips NaN, so the rule must be skipped explicitly
+    has_nan = __syncthreads_or(has_nan);
     bool kill_text = false;
-    if (apply_ts_rules && mx_ts > -INFINITY) {              // logsumexp over timestamps vs best text logit
+    if (apply_ts_rules && mx_ts > -INFINITY && !has_nan) {  // logsumexp over timestamps vs best text logit
         float s = 0.f;                                      // (evaluated BEFORE the silent-timestamp mask, as the
         for (int i = ts_begin + threadIdx.x; i < V; i += blockDim.x) s += expf(l[i] - mx_ts);   //  reference does)
         s = block_sum(s, red);
